@@ -16,7 +16,7 @@ BG_OK, BG_ERR_NULL, BG_ERR_INVALID, BG_ERR_CUDA, BG_ERR_CAPACITY, BG_ERR_UNSUPPO
 PASS_FORWARD, PASS_BACKWARD, PASS_BACKWARD_SMOOTH = 0, 1, 2
 PROJECTED_STRIDE = 16
 VCOMBINED_STRIDE = 10
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 _STATUS_NAMES = {1: "BG_ERR_NULL", 2: "BG_ERR_INVALID", 3: "BG_ERR_CUDA", 4: "BG_ERR_CAPACITY", 5: "BG_ERR_UNSUPPORTED"}
 
@@ -181,6 +181,11 @@ SIGNATURES = {
     "bg_render_forward": (_I32, [_P, _P, C.POINTER(BgCamera), _U32, _U32, _U32, _U32, _P, _P, _P, _I32,
                                  C.POINTER(_F), _I32, _P, _P, _P, C.POINTER(BgRenderState)]),
     "bg_rasterize_backward": (_I32, [_P, _P, C.POINTER(BgRenderState), _P, _P, C.POINTER(_F), _I32, _P, _U32]),
+    "bg_render_forward_depth": (_I32, [_P, _P, C.POINTER(BgCamera), _U32, _U32, _U32, _U32, _P, _P, _P, _I32,
+                                       C.POINTER(_F), _I32, _P, _P, _P, _P, C.POINTER(BgRenderState)]),
+    "bg_rasterize_backward_depth": (_I32, [_P, _P, C.POINTER(BgRenderState), _P, _P, _P, _P, C.POINTER(_F), _I32, _P, _U32, _P]),
+    "bg_project_backward_depth": (_I32, [_P, _P, C.POINTER(BgCamera), C.POINTER(BgRenderState), _P, _P, _P, _P, _P, _P, _P, _P,
+                                         _P]),
     "bg_debug_blend_stats": (_I32, [_P, _P, C.POINTER(BgRenderState), _P, _P, C.POINTER(_F), _P, _P]),
     "bg_project_backward": (_I32, [_P, _P, C.POINTER(BgCamera), C.POINTER(BgRenderState), _P, _P, _P, _P, _P, _P, _P, _P]),
     "bg_normal_noise": (_I32, [_P, _P, C.c_uint64, C.c_uint64, C.c_uint64, _P]),

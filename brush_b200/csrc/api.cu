@@ -39,14 +39,16 @@ cudaError_t launch_bump_epoch(cudaStream_t, uint32_t *);
 uint64_t sort_max_tiles(uint64_t n);
 // blend_fwd.cu / blend_bwd.cu
 cudaError_t launch_blend_fwd(cudaStream_t, bool, bool, uint32_t, const float *, const uint32_t *, uint32_t *, const uint32_t *,
-                             void *, float *, uint32_t *, uint32_t *, uint32_t, uint32_t, uint32_t, const float *);
+                             void *, float *, uint32_t *, uint32_t *, uint32_t, uint32_t, uint32_t, const float *, const float *,
+                             float *);
 cudaError_t launch_blend_bwd(cudaStream_t, bool, uint32_t, const float *, const uint32_t *, const uint32_t *, const float *,
                              const float *, const uint32_t *, const uint32_t *, float *, unsigned long long *, uint32_t,
-                             uint32_t, uint32_t, const float *);
+                             uint32_t, uint32_t, const float *, const float *, const float *, const float *, float *);
 // project_bwd.cu
 cudaError_t launch_project_bwd(cudaStream_t, bool, int, const float *, const float *, const float *,
                                const uint32_t *, const float *, uint32_t, const BgCamera &, float *, float *, float *,
                                float *, float *);
+cudaError_t launch_depth_to_means(cudaStream_t, const uint32_t *, const float *, uint32_t, const BgCamera &, float *);
 cudaError_t launch_normal_noise(cudaStream_t, uint64_t, uint64_t, uint64_t, float *);
 cudaError_t launch_train_fill_lr(cudaStream_t, float *, float *, uint32_t, float, float, float, float);
 cudaError_t launch_loss_reduce(cudaStream_t, const float *, uint32_t, uint32_t, const float *, float *);
@@ -120,6 +122,7 @@ struct BgContext {
     uint32_t *counters_host = nullptr;      // pinned [4]
     // last forward (for state pointers)
     int depth_out = 0, isect_out = 0;
+    bool depth_forward = false;   // the last forward also accumulated depth (bg_render_forward_depth)
 };
 
 // Launch indices inside one API call (each look-back chain of a call gets its own epoch).
@@ -237,10 +240,11 @@ static int32_t run_sort(BgContext *c, cudaStream_t s, const uint32_t *key_in, co
     return BG_OK;
 }
 
-extern "C" int32_t bg_render_forward(BgContext *c, void *stream, const BgCamera *cam, uint32_t w, uint32_t h,
-                                     uint32_t n, uint32_t k, const float *transforms, const float *sh,
-                                     const float *raw_opac, int32_t mip, const float *bg, int32_t pass, void *out_img,
-                                     float *visible, float *max_radius, BgRenderState *st) {
+// out_depth == nullptr: bg_render_forward; otherwise the depth forward (validated by bg_render_forward_depth)
+static int32_t render_forward(BgContext *c, void *stream, const BgCamera *cam, uint32_t w, uint32_t h, uint32_t n,
+                              uint32_t k, const float *transforms, const float *sh, const float *raw_opac, int32_t mip,
+                              const float *bg, int32_t pass, void *out_img, float *out_depth, float *visible,
+                              float *max_radius, BgRenderState *st) {
     if (!c || !cam || !bg || !out_img || !st) return BG_ERR_NULL;
     if (n > 0 && !max_radius) return BG_ERR_NULL;
     if (n > 0 && (!transforms || !sh || !raw_opac)) return BG_ERR_NULL;
@@ -260,6 +264,7 @@ extern "C" int32_t bg_render_forward(BgContext *c, void *stream, const BgCamera 
     if (n > c->max_n || num_tiles > c->max_tiles) { set_err("bg_render_forward: exceeds context capacity", cudaSuccess); return BG_ERR_CAPACITY; }
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
+    c->depth_forward = out_depth != nullptr;
 
     BG_CUDA(launch_bump_epoch(s, c->epoch_dev));
     BG_CUDA(cudaMemsetAsync(c->ctl, 0, CTL_WORDS * sizeof(uint32_t), s));
@@ -309,7 +314,8 @@ extern "C" int32_t bg_render_forward(BgContext *c, void *stream, const BgCamera 
     BG_CUDA(launch_tile_offsets(s, c->sm_count * 16, c->isect_key[iout], c->ctl, num_tiles, c->tile_offsets));
     // K5 (BG_PASS_BACKWARD_SMOOTH: the test-only smooth alpha cutoff of the finite-difference suites)
     BG_CUDA(launch_blend_fwd(s, bwd_info, pass == BG_PASS_BACKWARD_SMOOTH, num_tiles, c->projected, c->isect_val[iout],
-                             c->tile_offsets, gid_sorted, out_img, visible, c->live_masks, c->warp_batches, tiles_x, w, h, bg));
+                             c->tile_offsets, gid_sorted, out_img, visible, c->live_masks, c->warp_batches, tiles_x, w, h, bg,
+                             reinterpret_cast<const float *>(c->depth_key[dout]), out_depth));
     BG_CUDA(cudaMemcpyAsync(c->counters_host, counters, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
 
     st->projected = c->projected;
@@ -326,22 +332,75 @@ extern "C" int32_t bg_render_forward(BgContext *c, void *stream, const BgCamera 
     return BG_OK;
 }
 
-extern "C" int32_t bg_rasterize_backward(BgContext *c, void *stream, const BgRenderState *st, const float *out_img,
-                                         const float *v_output, const float *bg, int32_t smooth, float *v_combined,
-                                         uint32_t rows) {
-    if (!c || !st || !out_img || !v_output || !bg || !v_combined) return BG_ERR_NULL;
-    if (st->pass == BG_PASS_FORWARD) { set_err("bg_rasterize_backward requires a Backward pass state", cudaSuccess); return BG_ERR_INVALID; }
+extern "C" int32_t bg_render_forward(BgContext *c, void *stream, const BgCamera *cam, uint32_t w, uint32_t h,
+                                     uint32_t n, uint32_t k, const float *transforms, const float *sh,
+                                     const float *raw_opac, int32_t mip, const float *bg, int32_t pass, void *out_img,
+                                     float *visible, float *max_radius, BgRenderState *st) {
+    return render_forward(c, stream, cam, w, h, n, k, transforms, sh, raw_opac, mip, bg, pass, out_img, nullptr, visible,
+                          max_radius, st);
+}
+
+extern "C" int32_t bg_render_forward_depth(BgContext *c, void *stream, const BgCamera *cam, uint32_t w, uint32_t h,
+                                           uint32_t n, uint32_t k, const float *transforms, const float *sh,
+                                           const float *raw_opac, int32_t mip, const float *bg, int32_t pass,
+                                           float *out_img, float *out_depth, float *visible, float *max_radius,
+                                           BgRenderState *st) {
+    if (!out_depth) return BG_ERR_NULL;
+    if (pass != BG_PASS_BACKWARD && pass != BG_PASS_BACKWARD_SMOOTH) {
+        set_err("bg_render_forward_depth: depth needs an f32 pass (BG_PASS_BACKWARD or BG_PASS_BACKWARD_SMOOTH)", cudaSuccess);
+        return BG_ERR_INVALID;
+    }
+    if ((uintptr_t)out_depth % 4) { set_err("bg_render_forward_depth: out_depth must be 4-byte aligned", cudaSuccess); return BG_ERR_INVALID; }
+    return render_forward(c, stream, cam, w, h, n, k, transforms, sh, raw_opac, mip, bg, pass, out_img, out_depth, visible,
+                          max_radius, st);
+}
+
+// depth: out_depth / v_depth / v_z all set (bg_rasterize_backward_depth) or all null
+static int32_t rasterize_backward(BgContext *c, void *stream, const BgRenderState *st, const float *out_img,
+                                  const float *out_depth, const float *v_output, const float *v_depth, const float *bg,
+                                  int32_t smooth, float *v_combined, uint32_t rows, float *v_z, const char *who) {
+    auto invalid = [who](const char *what) {
+        char m[160];
+        snprintf(m, sizeof(m), "%s%s", who, what);
+        set_err(m, cudaSuccess);
+        return BG_ERR_INVALID;
+    };
+    if (st->pass == BG_PASS_FORWARD) return invalid(" requires a Backward pass state");
     const bool smooth_pass = st->pass == BG_PASS_BACKWARD_SMOOTH;
-    if ((smooth != 0) != smooth_pass) { set_err("bg_rasterize_backward: smooth_cutoff must match the state's pass", cudaSuccess); return BG_ERR_INVALID; }
-    if (st->tile_offsets != c->tile_offsets) { set_err("bg_rasterize_backward: needs the state of this context's last forward", cudaSuccess); return BG_ERR_INVALID; }
+    if ((smooth != 0) != smooth_pass) return invalid(": smooth_cutoff must match the state's pass");
+    if (st->tile_offsets != c->tile_offsets) return invalid(": needs the state of this context's last forward");
+    if (v_z && !c->depth_forward) return invalid(": this context's last forward did not render depth");
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
     const uint32_t zr = std::min(rows, std::max(st->n, 1u));
     BG_CUDA(cudaMemsetAsync(v_combined, 0, (size_t)zr * BG_VCOMBINED_STRIDE * sizeof(float), s));
+    if (v_z) BG_CUDA(cudaMemsetAsync(v_z, 0, (size_t)zr * sizeof(float), s));
     // the forward of this context left its hand-off words: replay exactly the splats it used
     BG_CUDA(launch_blend_bwd(s, smooth_pass, st->tiles_x * st->tiles_y, c->projected, st->compact_gid_from_isect, st->tile_offsets,
-                             out_img, v_output, c->live_masks, c->warp_batches, v_combined, nullptr, st->tiles_x, st->w, st->h, bg));
+                             out_img, v_output, c->live_masks, c->warp_batches, v_combined, nullptr, st->tiles_x, st->w, st->h, bg,
+                             st->depths, out_depth, v_depth, v_z));
     return BG_OK;
+}
+
+extern "C" int32_t bg_rasterize_backward(BgContext *c, void *stream, const BgRenderState *st, const float *out_img,
+                                         const float *v_output, const float *bg, int32_t smooth, float *v_combined,
+                                         uint32_t rows) {
+    if (!c || !st || !out_img || !v_output || !bg || !v_combined) return BG_ERR_NULL;
+    return rasterize_backward(c, stream, st, out_img, nullptr, v_output, nullptr, bg, smooth, v_combined, rows, nullptr,
+                              "bg_rasterize_backward");
+}
+
+extern "C" int32_t bg_rasterize_backward_depth(BgContext *c, void *stream, const BgRenderState *st, const float *out_img,
+                                               const float *out_depth, const float *v_output, const float *v_depth,
+                                               const float *bg, int32_t smooth, float *v_combined, uint32_t rows,
+                                               float *v_z) {
+    if (!c || !st || !out_img || !out_depth || !v_output || !v_depth || !bg || !v_combined || !v_z) return BG_ERR_NULL;
+    if (((uintptr_t)out_depth | (uintptr_t)v_depth | (uintptr_t)v_z) % 4) {
+        set_err("bg_rasterize_backward_depth: out_depth, v_depth and v_z must be 4-byte aligned", cudaSuccess);
+        return BG_ERR_INVALID;
+    }
+    return rasterize_backward(c, stream, st, out_img, out_depth, v_output, v_depth, bg, smooth, v_combined, rows, v_z,
+                              "bg_rasterize_backward_depth");
 }
 
 // Development counters of the blend loop for the last Backward-pass forward of this context:
@@ -358,7 +417,7 @@ extern "C" int32_t bg_debug_blend_stats(BgContext *c, void *stream, const BgRend
     BG_CUDA(cudaMemsetAsync(c->blend_stats, 0, 4 * sizeof(unsigned long long), s));
     BG_CUDA(launch_blend_bwd(s, false, st->tiles_x * st->tiles_y, c->projected, st->compact_gid_from_isect, st->tile_offsets, out_img,
                              v_output, c->live_masks, c->warp_batches, v_combined_scratch, c->blend_stats, st->tiles_x, st->w,
-                             st->h, bg));
+                             st->h, bg, nullptr, nullptr, nullptr, nullptr));
     BG_CUDA(cudaMemcpyAsync(out4, c->blend_stats, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
     BG_CUDA(cudaStreamSynchronize(s));
     out4[3] = st->counters_host ? st->counters_host[1] : 0;
@@ -382,6 +441,19 @@ extern "C" int32_t bg_project_backward(BgContext *c, void *stream, const BgCamer
     }
     BG_CUDA(launch_project_bwd(s, st->mip != 0, deg, transforms, sh, raw_opac, st->compact_from_global_gid, v_combined,
                                st->n, *cam, v_transforms, v_sh, v_raw_opac, v_refine, nullptr));
+    return BG_OK;
+}
+
+extern "C" int32_t bg_project_backward_depth(BgContext *c, void *stream, const BgCamera *cam, const BgRenderState *st,
+                                             const float *transforms, const float *sh, const float *raw_opac,
+                                             const float *v_combined, const float *v_z, float *v_transforms, float *v_sh,
+                                             float *v_raw_opac, float *v_refine) {
+    if (!v_z) return BG_ERR_NULL;
+    if ((uintptr_t)v_z % 4) { set_err("bg_project_backward_depth: v_z must be 4-byte aligned", cudaSuccess); return BG_ERR_INVALID; }
+    const int32_t r = bg_project_backward(c, stream, cam, st, transforms, sh, raw_opac, v_combined, v_transforms, v_sh,
+                                          v_raw_opac, v_refine);
+    if (r != BG_OK) return r;
+    BG_CUDA(launch_depth_to_means((cudaStream_t)stream, st->compact_from_global_gid, v_z, st->n, *cam, v_transforms));
     return BG_OK;
 }
 

@@ -22,6 +22,12 @@
 // v_alpha = d/d alpha already carries the factor w + alpha w'(alpha), and v_sigma = -alpha v_alpha with the raw alpha
 // (not alpha_eff) on the unsaturated pairs, so -(sum v_sigma)/opacity = sum e^-sigma v_alpha (rasterize_backwards.rs:349-372).
 // The 10 per-splat sums over the warp's 64 pixels are formed with a 12-shuffle reduce-scatter, one RED.F32 each.
+//
+// DEPTH: the adjoint of the accumulated depth D = sum vis_i z_i of a DEPTH forward (DESIGN §4.6).  Depth is one more
+// colour channel with colour z_i (no clamp, no gate, no background): the pixel state gains rem_d (initialised to the
+// final D) and v_D, the pair's v_alpha gains (T z_i - rem_d) v_D / (1 - alpha), and the 11th sum v_z_i = sum vis v_D
+// goes to the compact-indexed v_z[] (its factor, -1, sits in pad entry 10 of the factor row).  12 slots (slot 11 is
+// padding) cost one more shuffle in the first stage of the reduce-scatter.
 #include "blend_common.cuh"
 
 namespace bg {
@@ -33,13 +39,14 @@ __device__ __forceinline__ float rcp_approx_f(float x) { float r; asm("rcp.appro
 __device__ __forceinline__ float sqrt_approx_f(float x) { float r; asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
 
 // stats[0] warp-splat iterations, [1] pixel-splat pairs that blended, [2] pairs that stopped a pixel
-template <bool STATS, bool SMOOTH>
+template <bool STATS, bool SMOOTH, bool DEPTH>
 __global__ void __launch_bounds__(RASTER_THREADS)
 blend_bwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict__ cgid_from_isect,
                  const uint32_t *__restrict__ tile_offsets, const float4 *__restrict__ out_img,
                  const float4 *__restrict__ v_output, const uint32_t *__restrict__ live_masks,
                  const uint32_t *__restrict__ warp_batches, float *__restrict__ v_combined,
-                 unsigned long long *__restrict__ stats, BlendUniforms u) {
+                 unsigned long long *__restrict__ stats, BlendUniforms u, const float *__restrict__ depths,
+                 const float *__restrict__ out_depth, const float *__restrict__ v_depth, float *__restrict__ v_z) {
     __shared__ BlendStage s_stage[RASTER_WARPS];                         // per warp, double buffered rows (TMA destination)
     __shared__ __align__(16) float s_fact[RASTER_WARPS][2][WB * BFACT];  // post-reduction factors of the staged rows
 
@@ -83,12 +90,19 @@ blend_bwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
         load(inside0, pix_y0, T2.x, rem_r.x, rem_g.x, rem_b.x, vo_r.x, vo_g.x, vo_b.x, nvo_w.x, ifa.x);
         load(inside1, pix_y1, T2.y, rem_r.y, rem_g.y, rem_b.y, vo_r.y, vo_g.y, vo_b.y, nvo_w.y, ifa.y);
     }
+    float2 rem_d = make_float2(0.0f, 0.0f), vo_d = rem_d;   // depth still to come, v_D
+    if constexpr (DEPTH) {
+        const size_t pix0 = (size_t)pix_x + (size_t)pix_y0 * u.img_w, pix1 = (size_t)pix_x + (size_t)pix_y1 * u.img_w;
+        if (inside0) { rem_d.x = __ldg(out_depth + pix0); vo_d.x = __ldg(v_depth + pix0); }
+        if (inside1) { rem_d.y = __ldg(out_depth + pix1); vo_d.y = __ldg(v_depth + pix1); }
+    }
 
-    // reduce-scatter bookkeeping: which of the 10 sums this lane ends up owning
+    // reduce-scatter bookkeeping: which of the NS sums (10, or 12 with DEPTH) this lane ends up owning
+    constexpr int NS = DEPTH ? 12 : 10, NH = NS / 2;
     const bool b4 = lane & 16u, b3 = lane & 8u, b2 = lane & 4u, b1 = lane & 2u;
     const uint32_t idx5 = (b3 ? 3u : 0u) + (b2 ? 2u : 0u) + (b1 ? 1u : 0u);
-    const bool owner = !(lane & 1u) && !(b2 && b1) && !(b3 && b2);
-    const uint32_t slot = (b4 ? 5u : 0u) + idx5;
+    const uint32_t slot = (b4 ? (uint32_t)NH : 0u) + idx5;
+    const bool owner = !(lane & 1u) && !(b2 && b1) && (DEPTH ? slot != 11u : !(b3 && b2));
     const uint32_t lt_mask = (1u << lane) - 1u;
 
     const size_t mbase = blend_mask_base(range_lo, tile) + wid;
@@ -97,6 +111,8 @@ blend_bwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
     };
     // stage the rows of batch b selected by mask m, compacted in list order, into buffer b&1: the lanes park the row
     // ids, one elected lane issues the TMA copies
+    // (DEPTH: the same lane also starts the load of the row's z, which lands during the TMA wait)
+    float z_next = 0.0f;
     auto stage = [&](uint32_t b, uint32_t m) -> uint32_t {
         uint32_t id = 0;
         const uint32_t n = (uint32_t)__popc(m);
@@ -104,6 +120,7 @@ blend_bwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
         if ((m >> lane) & 1u) {
             id = __ldg(cgid_from_isect + range_lo + b * WB + lane);
             st.ids[b & 1u][__popc(m & lt_mask)] = id;
+            if constexpr (DEPTH) z_next = __ldg(depths + id);
         }
         stage_rows_tma(st, b & 1u, n, projected, lane);
         return id;
@@ -113,6 +130,7 @@ blend_bwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
     uint32_t id_next = stage(0, m_cur);
     for (uint32_t b = 0; b < num_batches; b++) {
         const uint32_t m = m_cur, my_id = id_next;
+        const float my_z = z_next;
         m_cur = m_next;
         m_next = load_mask(b + 2);
         id_next = stage(b + 1, m_cur);   // (an all-zero mask stages nothing)
@@ -137,6 +155,10 @@ blend_bwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
             *reinterpret_cast<float4 *>(f + 4) =
                 make_float4(-0.5f, B.z >= 0.0f ? -1.0f : 0.0f, B.w >= 0.0f ? -1.0f : 0.0f, bcol >= 0.0f ? -1.0f : 0.0f);
             *reinterpret_cast<float2 *>(f + 8) = make_float2(1.0f / B.y, 1.0f);
+            if constexpr (DEPTH) {
+                mine[ROW_Z] = my_z;
+                *reinterpret_cast<float2 *>(f + 10) = make_float2(-1.0f, 0.0f);   // the loop accumulates -v_z
+            }
         }
         __syncwarp();
         if (STATS) st_iter += n;
@@ -182,6 +204,12 @@ blend_bwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
             float2 nd = fmul2_rn(u_r, vo_r);
             nd = ffma2_rn(u_g, vo_g, nd);
             nd = ffma2_rn(u_b, vo_b, nd);                                   // -dot
+            float z = 0.0f;
+            if constexpr (DEPTH) {
+                z = row[ROW_Z];
+                const float2 u_d = ffma2_rn(T2, bcast2(-z), rem_d);          // rem_d - T z
+                nd = ffma2_rn(u_d, vo_d, nd);
+            }
             float2 nva = fmul2_rn(fadd2_rn(nd, nvo_w), ra);               // -v_alpha
             if constexpr (SMOOTH) nva = fmul2_rn(nva, make_float2(smooth_alpha_deriv(-nal.x), smooth_alpha_deriv(-nal.y)));
             const float2 nvs = fmul2_rn(nals, nva);                         // -v_sigma  (= alpha v_alpha)
@@ -195,20 +223,27 @@ blend_bwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
             rem_r = ffma2_rn(nvis, bcast2(B.z), rem_r);
             rem_g = ffma2_rn(nvis, bcast2(B.w), rem_g);
             rem_b = ffma2_rn(nvis, bcast2(C.x), rem_b);
+            float2 G10 = make_float2(0.0f, 0.0f);
+            if constexpr (DEPTH) {
+                G10 = fmul2_rn(nvis, vo_d);                                  // -vis v_D
+                rem_d = ffma2_rn(nvis, bcast2(z), rem_d);
+            }
             T2.x = act0 ? nT.x : T2.x;
             T2.y = act1 ? nT.y : T2.y;
-            // ---- the lane's two pixels, then reduce-scatter 10 values over 32 lanes: 5+3+2+1+1 shuffles
-            float g[10];
+            // ---- the lane's two pixels, then reduce-scatter NS values over 32 lanes: 5+3+2+1+1 shuffles (6+3+2+1+1
+            // with DEPTH, whose 12 values fill the sixth entry that is padding otherwise)
+            float g[NS];
             g[0] = G0.x + G0.y; g[1] = G1.x + G1.y; g[2] = G2.x + G2.y; g[3] = G3.x + G3.y; g[4] = G4.x + G4.y;
             g[5] = G5.x + G5.y; g[6] = G6.x + G6.y; g[7] = G7.x + G7.y; g[8] = nvs.x + nvs.y; g[9] = G9.x + G9.y;
+            if constexpr (DEPTH) { g[10] = G10.x + G10.y; g[11] = 0.0f; }
             float a5[6];
 #pragma unroll
-            for (int i = 0; i < 5; i++) {
-                float send = b4 ? g[i] : g[i + 5];
-                float keep = b4 ? g[i + 5] : g[i];
+            for (int i = 0; i < NH; i++) {
+                float send = b4 ? g[i] : g[i + NH];
+                float keep = b4 ? g[i + NH] : g[i];
                 a5[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
             }
-            a5[5] = 0.0f;
+            if constexpr (!DEPTH) a5[5] = 0.0f;
             float b3v[4];
 #pragma unroll
             for (int i = 0; i < 3; i++) {
@@ -233,7 +268,8 @@ blend_bwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
             d1 += __shfl_xor_sync(0xffffffffu, d1, 1);
             if (owner && d1 != 0.0f) {
                 const uint32_t id = __float_as_uint(row[BROW_ID]);
-                atomicAdd(v_combined + (size_t)id * BG_VCOMBINED_STRIDE + slot, d1 * fact[j * BFACT + slot]);
+                if (DEPTH && slot == 10u) atomicAdd(v_z + id, d1 * fact[j * BFACT + slot]);
+                else atomicAdd(v_combined + (size_t)id * BG_VCOMBINED_STRIDE + slot, d1 * fact[j * BFACT + slot]);
             }
         }
         __syncwarp();  // all lanes are done with this buffer before the next stage() overwrites it
@@ -246,20 +282,26 @@ blend_bwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
 cudaError_t launch_blend_bwd(cudaStream_t s, bool smooth, uint32_t num_tiles, const float *projected, const uint32_t *cgid_from_isect,
                              const uint32_t *tile_offsets, const float *out_img, const float *v_output, const uint32_t *live_masks,
                              const uint32_t *warp_batches, float *v_combined, unsigned long long *stats, uint32_t tiles_x,
-                             uint32_t w, uint32_t h, const float *bg) {
+                             uint32_t w, uint32_t h, const float *bg, const float *depths, const float *out_depth,
+                             const float *v_depth, float *v_z) {
     BlendUniforms u;
     u.tiles_x = tiles_x; u.img_w = w; u.img_h = h; u.bg_r = bg[0]; u.bg_g = bg[1]; u.bg_b = bg[2];
-    if (smooth)   // (test-only: no counting variant)
-        blend_bwd_kernel<false, true><<<num_tiles, RASTER_THREADS, 0, s>>>(projected, cgid_from_isect, tile_offsets, (const float4 *)out_img,
-                                                                           (const float4 *)v_output, live_masks, warp_batches, v_combined,
-                                                                           nullptr, u);
-    else if (stats)
-        blend_bwd_kernel<true, false><<<num_tiles, RASTER_THREADS, 0, s>>>(projected, cgid_from_isect, tile_offsets, (const float4 *)out_img,
-                                                                           (const float4 *)v_output, live_masks, warp_batches, v_combined, stats, u);
-    else
-        blend_bwd_kernel<false, false><<<num_tiles, RASTER_THREADS, 0, s>>>(projected, cgid_from_isect, tile_offsets, (const float4 *)out_img,
-                                                                            (const float4 *)v_output, live_masks, warp_batches, v_combined,
-                                                                            nullptr, u);
+#define BG_LAUNCH_BWD(ST, S, D, STATS_PTR)                                                                                \
+    blend_bwd_kernel<ST, S, D><<<num_tiles, RASTER_THREADS, 0, s>>>(projected, cgid_from_isect, tile_offsets, (const float4 *)out_img, \
+                                                                    (const float4 *)v_output, live_masks, warp_batches, v_combined, \
+                                                                    STATS_PTR, u, depths, out_depth, v_depth, v_z)
+    // (test-only smooth cutoff and the depth adjoint: no counting variant)
+    if (v_z) {
+        if (smooth) BG_LAUNCH_BWD(false, true, true, nullptr);
+        else BG_LAUNCH_BWD(false, false, true, nullptr);
+    } else if (smooth) {
+        BG_LAUNCH_BWD(false, true, false, nullptr);
+    } else if (stats) {
+        BG_LAUNCH_BWD(true, false, false, stats);
+    } else {
+        BG_LAUNCH_BWD(false, false, false, nullptr);
+    }
+#undef BG_LAUNCH_BWD
     return cudaGetLastError();
 }
 

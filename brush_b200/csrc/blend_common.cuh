@@ -35,6 +35,7 @@ constexpr int RASTER_THREADS = RASTER_WARPS * 32;
 constexpr int WB = 32;                    // splats per warp batch
 constexpr int ROW = BG_PROJECTED_STRIDE;  // 16 floats
 constexpr int ROW_PT = 12;                // lane of ln(255 opacity), the block-cull threshold
+constexpr int ROW_Z = 13;                 // pad lane that the DEPTH variants fill with the splat's camera-space z
 
 struct BlendUniforms {
     uint32_t tiles_x, img_w, img_h;

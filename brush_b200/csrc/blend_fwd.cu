@@ -6,6 +6,9 @@
 // With BWD_INFO: rgba f32 output, visible[gid] = 1 for every blended splat, the tile's range end trimmed to one
 // past the last blended splat (rasterize.rs:183-189), and the hand-off words of blend_common.cuh.
 // SMOOTH (test-only, BWD_INFO only): the smooth alpha cutoff of blend_common.cuh, and its wider block-cull margin.
+// DEPTH (BWD_INFO only): also the accumulated depth D = sum vis_i z_i ([h,w] f32, no background term; DESIGN §4.6),
+// z_i = depths[compact id], the depth-sort key.  The staging lane parks z_i in pad lane 13 of the row; every other
+// output (image, visible, trimmed ends, hand-off words) is the same as without DEPTH.
 //
 // Bound: instruction issue (FP32 + MUFU), not HBM.  Per warp-splat iteration (64 pixel-splat pairs) the loop is
 // 3 broadcast LDS.128, 4 scalar + 9 paired (18 scalar) FMA-pipe operations, 2 MUFU.EX2 and the pair tests.  The rows of a
@@ -14,12 +17,13 @@
 
 namespace bg {
 
-template <bool BWD_INFO, bool SMOOTH>
+template <bool BWD_INFO, bool SMOOTH, bool DEPTH>
 __global__ void __launch_bounds__(RASTER_THREADS)
 blend_fwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict__ cgid_from_isect,
                  uint32_t *__restrict__ tile_offsets, const uint32_t *__restrict__ gid_from_cgid,
                  float4 *__restrict__ out_f32, uint32_t *__restrict__ out_packed, float *__restrict__ visible,
-                 uint32_t *__restrict__ live_masks, uint32_t *__restrict__ warp_batches, BlendUniforms u) {
+                 uint32_t *__restrict__ live_masks, uint32_t *__restrict__ warp_batches, BlendUniforms u,
+                 const float *__restrict__ depths, float *__restrict__ out_depth) {
     __shared__ BlendStage s_stage[RASTER_WARPS];   // per warp, double buffered
     __shared__ uint32_t s_max_useful;
 
@@ -46,19 +50,21 @@ blend_fwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
     // the stopping splat's T' (<= 1e-4) afterwards, so that "T' > 1e-4" alone rejects every later splat.
     float2 T2 = make_float2(1.0f, 1.0f);
     float2 Tt2 = make_float2(inside0 ? 1.0f : 0.0f, inside1 ? 1.0f : 0.0f);
-    float2 r2 = make_float2(0.0f, 0.0f), g2 = r2, b2 = r2;
+    float2 r2 = make_float2(0.0f, 0.0f), g2 = r2, b2 = r2, d2 = r2;
     uint32_t last_useful = range_lo;
 
     const uint32_t num_batches = (range_hi - range_lo + WB - 1) / WB;
     const size_t mbase = blend_mask_base(range_lo, tile) + wid;
     uint32_t batches_walked = 0;
     uint32_t next_id = 0;
+    float next_z = 0.0f;
     // stage batch b: every lane parks the id of "its" list entry, one elected lane issues the TMA copies
     auto prefetch = [&](uint32_t b) {
         const uint32_t start = range_lo + b * WB;
         const uint32_t count = min((uint32_t)WB, range_hi - start);
         const uint32_t id = lane < count ? __ldg(cgid_from_isect + start + lane) : 0u;
         next_id = id;
+        if constexpr (DEPTH) next_z = lane < count ? __ldg(depths + id) : 0.0f;   // in flight during the TMA wait
         if (lane < count) st.ids[b & 1u][lane] = id;
         stage_rows_tma(st, b & 1u, count, projected, lane);
     };
@@ -69,6 +75,7 @@ blend_fwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
             const uint32_t batch_start = range_lo + b * WB;
             const uint32_t count = min((uint32_t)WB, range_hi - batch_start);
             const uint32_t my_id = next_id;
+            const float my_z = next_z;
             if (b + 1 < num_batches) prefetch(b + 1);
             mbar_wait(&st.bar[b & 1u], (phase_bits >> (b & 1u)) & 1u);
             phase_bits ^= 1u << (b & 1u);
@@ -85,6 +92,7 @@ blend_fwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
                 // per-splat constants are formed once here, by the lane that staged the row: colour -> max(colour, 0)
                 *reinterpret_cast<float2 *>(mine + 6) = make_float2(fmaxf(B.z, 0.0f), fmaxf(B.w, 0.0f));
                 mine[8] = fmaxf(bcol, 0.0f);
+                if constexpr (DEPTH) mine[ROW_Z] = my_z;
             }
             uint32_t bits = __ballot_sync(0xffffffffu, hit);   // (also orders the row fix-ups before the reads below)
             uint32_t used_m = 0, acted_m = 0;
@@ -117,6 +125,7 @@ blend_fwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
                 r2 = ffma2_rn(bcast2(B.z), vis, r2);
                 g2 = ffma2_rn(bcast2(B.w), vis, g2);
                 b2 = ffma2_rn(bcast2(C.x), vis, b2);
+                if constexpr (DEPTH) d2 = ffma2_rn(bcast2(row[ROW_Z]), vis, d2);
                 const uint32_t bit = 1u << s;
                 // the hand-off needs the splats that changed a live pixel: blended it or stopped it
                 const bool acted = (Tt2.x > 1.0e-4f && act0) || (Tt2.y > 1.0e-4f && act1);
@@ -145,11 +154,12 @@ blend_fwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
         }
     }
 
-    auto write_pixel = [&](float T, float r, float g, float bl, uint32_t pix_y) {
+    auto write_pixel = [&](float T, float r, float g, float bl, float d, uint32_t pix_y) {
         const float fr = r + T * u.bg_r, fg = g + T * u.bg_g, fb = bl + T * u.bg_b, fa = 1.0f - T;
         const size_t pix_id = (size_t)pix_x + (size_t)pix_y * u.img_w;
         if (BWD_INFO) {
             out_f32[pix_id] = make_float4(fr, fg, fb, fa);
+            if constexpr (DEPTH) out_depth[pix_id] = d;
         } else {
             uint32_t r8 = (uint32_t)fminf(fmaxf(fr * 255.0f, 0.0f), 255.0f);
             uint32_t g8 = (uint32_t)fminf(fmaxf(fg * 255.0f, 0.0f), 255.0f);
@@ -158,8 +168,8 @@ blend_fwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
             out_packed[pix_id] = r8 | (g8 << 8) | (b8 << 16) | (a8 << 24);
         }
     };
-    if (inside0) write_pixel(T2.x, r2.x, g2.x, b2.x, pix_y0);
-    if (inside1) write_pixel(T2.y, r2.y, g2.y, b2.y, pix_y1);
+    if (inside0) write_pixel(T2.x, r2.x, g2.x, b2.x, d2.x, pix_y0);
+    if (inside1) write_pixel(T2.y, r2.y, g2.y, b2.y, d2.y, pix_y1);
     if (BWD_INFO) {
         if (lane == 0) warp_batches[tile * RASTER_WARPS + wid] = batches_walked;
         // one block barrier, after all blending: publish the trimmed range end
@@ -175,18 +185,23 @@ blend_fwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
 cudaError_t launch_blend_fwd(cudaStream_t s, bool bwd_info, bool smooth, uint32_t num_tiles, const float *projected,
                              const uint32_t *cgid_from_isect, uint32_t *tile_offsets, const uint32_t *gid_from_cgid, void *out_img,
                              float *visible, uint32_t *live_masks, uint32_t *warp_batches, uint32_t tiles_x, uint32_t w,
-                             uint32_t h, const float *bg) {
+                             uint32_t h, const float *bg, const float *depths, float *out_depth) {
     BlendUniforms u;
     u.tiles_x = tiles_x; u.img_w = w; u.img_h = h; u.bg_r = bg[0]; u.bg_g = bg[1]; u.bg_b = bg[2];
+#define BG_LAUNCH_FWD(B, S, D, F32, PACKED, LM, WBAT)                                                                    \
+    blend_fwd_kernel<B, S, D><<<num_tiles, RASTER_THREADS, 0, s>>>(projected, cgid_from_isect, tile_offsets, gid_from_cgid, \
+                                                                   F32, PACKED, visible, LM, WBAT, u, depths, out_depth)
     if (!bwd_info)
-        blend_fwd_kernel<false, false><<<num_tiles, RASTER_THREADS, 0, s>>>(projected, cgid_from_isect, tile_offsets, gid_from_cgid,
-                                                                            nullptr, (uint32_t *)out_img, visible, nullptr, nullptr, u);
+        BG_LAUNCH_FWD(false, false, false, nullptr, (uint32_t *)out_img, nullptr, nullptr);
+    else if (out_depth && !smooth)   // (depth with bwd_info only: the entry point rejects it for the packed pass)
+        BG_LAUNCH_FWD(true, false, true, (float4 *)out_img, nullptr, live_masks, warp_batches);
+    else if (out_depth)
+        BG_LAUNCH_FWD(true, true, true, (float4 *)out_img, nullptr, live_masks, warp_batches);
     else if (!smooth)
-        blend_fwd_kernel<true, false><<<num_tiles, RASTER_THREADS, 0, s>>>(projected, cgid_from_isect, tile_offsets, gid_from_cgid,
-                                                                           (float4 *)out_img, nullptr, visible, live_masks, warp_batches, u);
+        BG_LAUNCH_FWD(true, false, false, (float4 *)out_img, nullptr, live_masks, warp_batches);
     else
-        blend_fwd_kernel<true, true><<<num_tiles, RASTER_THREADS, 0, s>>>(projected, cgid_from_isect, tile_offsets, gid_from_cgid,
-                                                                          (float4 *)out_img, nullptr, visible, live_masks, warp_batches, u);
+        BG_LAUNCH_FWD(true, true, false, (float4 *)out_img, nullptr, live_masks, warp_batches);
+#undef BG_LAUNCH_FWD
     return cudaGetLastError();
 }
 

@@ -390,4 +390,30 @@ cudaError_t launch_project_bwd(cudaStream_t s, bool mip, int deg, const float *t
                                       v_sh, v_raw_opac, v_refine, v_color_out);
 }
 
+// Depth adjoint, after project_bwd_kernel (DESIGN §4.6): z_i = R[2,:] . mean_i + t_z, so the blend's v_z[cgid] adds
+// v_z R[2,:] to v_transforms[gid, 0:3].  Every Gaussian owns its row: no atomics, deterministic.  A zero v_z leaves the
+// row's bits as they are (adding +0 would turn a -0 into +0).
+__global__ void __launch_bounds__(256)
+depth_to_means_kernel(const uint32_t *__restrict__ cgid_from_gid, const float *__restrict__ v_z, uint32_t n, float r0,
+                      float r1, float r2, float *__restrict__ v_transforms) {
+    const uint32_t gid = blockIdx.x * 256u + threadIdx.x;
+    if (gid >= n) return;
+    const uint32_t cg = __ldg(cgid_from_gid + gid);
+    if (cg == 0xFFFFFFFFu) return;
+    const float vz = __ldg(v_z + cg);
+    if (vz == 0.0f) return;
+    float *t = v_transforms + (size_t)gid * 10;
+    t[0] += vz * r0;
+    t[1] += vz * r1;
+    t[2] += vz * r2;
+}
+
+cudaError_t launch_depth_to_means(cudaStream_t s, const uint32_t *cgid_from_gid, const float *v_z, uint32_t n,
+                                  const BgCamera &u, float *v_transforms) {
+    if (n == 0) return cudaSuccess;
+    depth_to_means_kernel<<<(n + 255) / 256, 256, 0, s>>>(cgid_from_gid, v_z, n, u.viewmat[2], u.viewmat[5], u.viewmat[8],
+                                                          v_transforms);
+    return cudaGetLastError();
+}
+
 }  // namespace bg

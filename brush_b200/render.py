@@ -4,6 +4,8 @@
                                    (brush-render/src/lib.rs:54-77, render_aux.rs:16-81)
   rasterize_bwd / project_bwd   <- SplatBwdOps (brush-render/src/bwd/burn_glue.rs:62-92)
   RenderFunction                <- RenderBackwards (bwd/burn_glue.rs:121-182): autograd glue
+  render_splats(render_depth=True), rasterize_bwd_depth, project_bwd(v_z=...), RenderDepthFunction,
+  expected_depth                <- differentiable per-pixel depth (DESIGN.md section 4.6; no reference operator)
 
 PyTorch supplies device memory and the current stream only; all compute goes through
 libbrush_b200.so (brush_b200/_lib.py).  No CPU path exists.
@@ -91,6 +93,7 @@ class RenderOutput:
     background: Tuple[float, float, float]
     ctx: RenderContext
     _event: torch.cuda.Event = field(default=None, repr=False)
+    depth: Optional[torch.Tensor] = None  # [h,w] f32 accumulated depth sum_i vis_i z_i (render_depth=True only)
 
     def _counters(self):
         if self._event is not None:
@@ -139,9 +142,12 @@ class RenderOutput:
 
 def render_splats(ctx: RenderContext, camera, img_size, transforms: torch.Tensor, sh_coeffs: torch.Tensor,
                   raw_opacities: torch.Tensor, mip: bool = False, background=(0.0, 0.0, 0.0),
-                  rpass: int = PASS_BACKWARD) -> RenderOutput:
+                  rpass: int = PASS_BACKWARD, render_depth: bool = False) -> RenderOutput:
     """<MainBackendBase as SplatOps>::render (render.rs:37-315).  img_size = (w, h).
-    `camera` is a brush_b200.camera.Camera or prebuilt ProjectUniforms."""
+    `camera` is a brush_b200.camera.Camera or prebuilt ProjectUniforms.
+    render_depth: also return `depth`, the [h,w] accumulated depth sum_i alpha_i T_i z_i (z_i = camera-space z of the
+    splat mean; no background term).  Needs an f32 pass (PASS_BACKWARD or PASS_BACKWARD_SMOOTH); expected_depth()
+    turns it into the expected depth."""
     lib = _lib.load()
     w, h = int(img_size[0]), int(img_size[1])
     transforms = _f32c(transforms, "transforms")
@@ -165,18 +171,29 @@ def render_splats(ctx: RenderContext, camera, img_size, transforms: torch.Tensor
     max_radius = torch.empty((n,), dtype=torch.float32, device=dev)
     bg = (C.c_float * 3)(*[float(b) for b in background])
     st = _lib.BgRenderState()
-    _lib.check(
-        lib.bg_render_forward(ctx.handle, _stream_ptr(dev), C.byref(cam), w, h, n, k, transforms.data_ptr(),
-                              sh_coeffs.data_ptr(), raw_opacities.data_ptr(), int(bool(mip)), bg, int(rpass),
-                              out_img.data_ptr(), visible.data_ptr() if visible is not None else None,
-                              max_radius.data_ptr(), C.byref(st)),
-        "bg_render_forward")
+    depth = None
+    if render_depth:
+        depth = torch.empty((h, w), dtype=torch.float32, device=dev)
+        _lib.check(
+            lib.bg_render_forward_depth(ctx.handle, _stream_ptr(dev), C.byref(cam), w, h, n, k, transforms.data_ptr(),
+                                        sh_coeffs.data_ptr(), raw_opacities.data_ptr(), int(bool(mip)), bg, int(rpass),
+                                        out_img.data_ptr(), depth.data_ptr(),
+                                        visible.data_ptr() if visible is not None else None, max_radius.data_ptr(),
+                                        C.byref(st)),
+            "bg_render_forward_depth")
+    else:
+        _lib.check(
+            lib.bg_render_forward(ctx.handle, _stream_ptr(dev), C.byref(cam), w, h, n, k, transforms.data_ptr(),
+                                  sh_coeffs.data_ptr(), raw_opacities.data_ptr(), int(bool(mip)), bg, int(rpass),
+                                  out_img.data_ptr(), visible.data_ptr() if visible is not None else None,
+                                  max_radius.data_ptr(), C.byref(st)),
+            "bg_render_forward")
     ev = None
     if not torch.cuda.is_current_stream_capturing():
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream(dev))
     return RenderOutput(out_img=out_img, visible=visible, max_radius=max_radius, state=st, cam=cam, uniforms=uniforms,
-                        background=tuple(float(b) for b in background), ctx=ctx, _event=ev)
+                        background=tuple(float(b) for b in background), ctx=ctx, _event=ev, depth=depth)
 
 
 def rasterize_bwd(out: RenderOutput, v_output: torch.Tensor, smooth_cutoff: Optional[bool] = None) -> torch.Tensor:
@@ -199,6 +216,33 @@ def rasterize_bwd(out: RenderOutput, v_output: torch.Tensor, smooth_cutoff: Opti
     return v_combined
 
 
+def rasterize_bwd_depth(out: RenderOutput, v_output: torch.Tensor, v_depth: torch.Tensor):
+    """Adjoint of a render_depth=True render: rasterize_bwd with the upstream gradient v_depth [h,w] of out.depth.
+    Returns (v_combined [n,10], v_z [n]); v_z is indexed by compact id like v_combined and feeds project_bwd(v_z=...).
+    `out` must still be its context's last render."""
+    lib = _lib.load()
+    v_output = _f32c(v_output, "v_output")
+    v_depth = _f32c(v_depth, "v_depth")
+    st = out.state
+    if tuple(v_output.shape) != (st.h, st.w, 4):
+        raise ValueError("v_output must be [h, w, 4]")
+    if tuple(v_depth.shape) != (st.h, st.w):
+        raise ValueError("v_depth must be [h, w]")
+    if out.depth is None:
+        raise ValueError("rasterize_bwd_depth needs a render_splats(..., render_depth=True) output")
+    rows = max(int(st.n), 1)
+    v_combined = torch.empty((rows, VCOMBINED_STRIDE), dtype=torch.float32, device=out.ctx.device)
+    v_z = torch.empty((rows,), dtype=torch.float32, device=out.ctx.device)
+    bg = (C.c_float * 3)(*out.background)
+    _lib.check(
+        lib.bg_rasterize_backward_depth(out.ctx.handle, _stream_ptr(out.ctx.device), C.byref(st), out.out_img.data_ptr(),
+                                        out.depth.data_ptr(), v_output.data_ptr(), v_depth.data_ptr(), bg,
+                                        int(st.pass_ == PASS_BACKWARD_SMOOTH), v_combined.data_ptr(), rows,
+                                        v_z.data_ptr()),
+        "bg_rasterize_backward_depth")
+    return v_combined, v_z
+
+
 def blend_stats(out: RenderOutput, v_output: torch.Tensor) -> dict:
     """Measurement aid (bg_debug_blend_stats): counters of the blend loop for `out` (a PASS_BACKWARD render that is
     still this context's last forward).  Synchronises the stream."""
@@ -216,10 +260,11 @@ def blend_stats(out: RenderOutput, v_output: torch.Tensor) -> dict:
             "pairs_stopping": stop, "lane_utilisation": (live / (it * 64)) if it else 0.0}
 
 
-def project_bwd(out: RenderOutput, transforms, sh_coeffs, raw_opacities, v_combined, outputs=None):
+def project_bwd(out: RenderOutput, transforms, sh_coeffs, raw_opacities, v_combined, outputs=None, v_z=None):
     """SplatBwdOps::project_bwd (bwd/render_bwd.rs:102-171) -> (v_transforms, v_coeffs, v_raw_opac, v_refine_weight).
     `outputs`: optional preallocated (v_t [n,10], v_sh [n,k,3], v_o [n], v_r [n]) -- e.g. views of one flat
-    buffer so that data-parallel training can all-reduce all gradients with a single collective."""
+    buffer so that data-parallel training can all-reduce all gradients with a single collective.
+    `v_z`: the depth gradient of rasterize_bwd_depth; its chain to the means is added to v_transforms[:, 0:3]."""
     lib = _lib.load()
     transforms = _f32c(transforms, "transforms")
     sh_coeffs = _f32c(sh_coeffs, "sh_coeffs")
@@ -237,11 +282,22 @@ def project_bwd(out: RenderOutput, transforms, sh_coeffs, raw_opacities, v_combi
         v_sh = torch.empty((n, k, 3), dtype=torch.float32, device=dev)
         v_o = torch.empty((n,), dtype=torch.float32, device=dev)
         v_r = torch.empty((n,), dtype=torch.float32, device=dev)
-    _lib.check(
-        lib.bg_project_backward(out.ctx.handle, _stream_ptr(dev), C.byref(out.cam), C.byref(out.state),
-                                transforms.data_ptr(), sh_coeffs.data_ptr(), raw_opacities.data_ptr(),
-                                v_combined.data_ptr(), v_t.data_ptr(), v_sh.data_ptr(), v_o.data_ptr(), v_r.data_ptr()),
-        "bg_project_backward")
+    if v_z is None:
+        _lib.check(
+            lib.bg_project_backward(out.ctx.handle, _stream_ptr(dev), C.byref(out.cam), C.byref(out.state),
+                                    transforms.data_ptr(), sh_coeffs.data_ptr(), raw_opacities.data_ptr(),
+                                    v_combined.data_ptr(), v_t.data_ptr(), v_sh.data_ptr(), v_o.data_ptr(), v_r.data_ptr()),
+            "bg_project_backward")
+    else:
+        v_z = _f32c(v_z, "v_z")
+        if v_z.dim() != 1 or v_z.shape[0] < max(n, 1):
+            raise ValueError("v_z must be [n] (as returned by rasterize_bwd_depth)")
+        _lib.check(
+            lib.bg_project_backward_depth(out.ctx.handle, _stream_ptr(dev), C.byref(out.cam), C.byref(out.state),
+                                          transforms.data_ptr(), sh_coeffs.data_ptr(), raw_opacities.data_ptr(),
+                                          v_combined.data_ptr(), v_z.data_ptr(), v_t.data_ptr(), v_sh.data_ptr(),
+                                          v_o.data_ptr(), v_r.data_ptr()),
+            "bg_project_backward_depth")
     return v_t, v_sh, v_o, v_r
 
 
@@ -323,6 +379,41 @@ class RenderFunction(torch.autograd.Function):
         # refine_weight_holder is an [n] tensor here (torch requires matching shapes); its gradient is
         # v_refine_weight, exactly what the reference registers on its holder node.
         return v_t, v_sh, v_o, v_r, None, None, None, None, None, None
+
+
+class RenderDepthFunction(torch.autograd.Function):
+    """RenderFunction with the accumulated depth as a second differentiable output: forward returns
+    (img, depth, visible, max_radius).  When no gradient reaches `depth`, backward is RenderFunction's."""
+
+    @staticmethod
+    def forward(fctx, transforms, sh_coeffs, raw_opacities, refine_weight_holder, ctx, camera, img_size, mip, background,
+                rpass):
+        out = render_splats(ctx, camera, img_size, transforms, sh_coeffs, raw_opacities, mip, background, rpass,
+                            render_depth=True)
+        fctx.out = out
+        fctx.save_for_backward(transforms, sh_coeffs, raw_opacities)
+        fctx.mark_non_differentiable(out.visible, out.max_radius)
+        fctx.set_materialize_grads(False)
+        return out.out_img, out.depth, out.visible, out.max_radius
+
+    @staticmethod
+    def backward(fctx, v_img, v_depth, _v_vis, _v_rad):
+        transforms, sh_coeffs, raw_opacities = fctx.saved_tensors
+        out = fctx.out
+        if v_img is None:
+            v_img = torch.zeros_like(out.out_img)
+        if v_depth is None:
+            v_combined, v_z = rasterize_bwd(out, v_img.contiguous()), None
+        else:
+            v_combined, v_z = rasterize_bwd_depth(out, v_img.contiguous(), v_depth.contiguous())
+        v_t, v_sh, v_o, v_r = project_bwd(out, transforms, sh_coeffs, raw_opacities, v_combined, v_z=v_z)
+        return v_t, v_sh, v_o, v_r, None, None, None, None, None, None
+
+
+def expected_depth(img: torch.Tensor, depth: torch.Tensor, eps: float = 1e-10) -> torch.Tensor:
+    """Expected depth D / alpha of a depth render (alpha = img[..., 3]); differentiable through both inputs.
+    Pixels that nothing covers (alpha <= eps) divide by eps, giving ~0 since D is 0 there too."""
+    return depth / img[..., 3].clamp_min(eps)
 
 
 def radix_argsort(ctx: RenderContext, keys: torch.Tensor, values: torch.Tensor, sorting_bits: int):

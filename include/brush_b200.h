@@ -35,13 +35,14 @@
 extern "C" {
 #endif
 
-#define BG_ABI_VERSION 5u
+#define BG_ABI_VERSION 6u
 
 /* f32 lanes per projected splat: a 64-byte row, four aligned 128-bit loads.  Lanes 0..8 are the reference
  * layout (kernels/helpers.rs:49-53: xy_x, xy_y, conic_x, conic_y, conic_z, color_a, color_r, color_g, color_b).
  * Lanes 9..12 are derived values cached for the blend kernels: 9 = log2(e)/2 * conic_z, 10 = log2(e)/2 * conic_x,
  * 11 = log2(e) * conic_y (so that alpha = opacity * 2^-(l10 dx^2 + l9 dy^2 + l11 dx dy) costs three FMA-class
- * operations and one MUFU per pixel), 12 = ln(255 * opacity) (the block-cull threshold); 13..15 pad. */
+ * operations and one MUFU per pixel), 12 = ln(255 * opacity) (the block-cull threshold); 13..15 pad (the blend
+ * kernels' shared-memory copy of a row carries the splat's depth in lane 13 when depth is rendered). */
 #define BG_PROJECTED_STRIDE 16u
 /* f32 lanes per row of v_combined (bwd/burn_glue.rs:36-43). */
 #define BG_VCOMBINED_STRIDE 10u
@@ -140,6 +141,38 @@ int32_t bg_render_forward(BgContext *ctx, void *stream, const BgCamera *cam, uin
 int32_t bg_rasterize_backward(BgContext *ctx, void *stream, const BgRenderState *state, const float *out_img,
                               const float *v_output, const float *bg, int32_t smooth_cutoff,
                               float *v_combined, uint32_t v_combined_rows);
+
+/* ---- Differentiable depth (DESIGN.md §4.6; no reference operator).
+ * bg_render_forward_depth is bg_render_forward for the f32 passes (BG_PASS_BACKWARD, BG_PASS_BACKWARD_SMOOTH;
+ * BG_PASS_FORWARD is BG_ERR_INVALID) that also writes the accumulated depth
+ *     out_depth[y,x] = D = sum_i vis_i z_i          (device [h,w] f32)
+ * with vis_i = alpha_i T_i the weight the colour uses (same cutoffs, the stopping splat not blended) and z_i the
+ * splat mean's camera-space z (the depth-sort key, state->depths).  There is no background term; the expected depth
+ * is D / out_img[y,x,3], formed by the caller.  out_img, visible, max_radius, the state and the tile ranges are
+ * bit-identical to bg_render_forward's.
+ * bg_rasterize_backward_depth is bg_rasterize_backward with the upstream gradient v_depth [h,w] of D: depth enters
+ * v_alpha like a fourth colour channel with colour z_i, so v_combined also carries the depth terms (its refine weight
+ * is formed from the total screen-space gradient), and v_z (device [v_combined_rows]) receives
+ * v_z[cgid] = sum over pixels of vis v_depth, indexed by compact id like v_combined; its first min(rows, n) entries
+ * are zeroed here.  Besides the preconditions of bg_rasterize_backward, the state must come from this context's last
+ * forward AND that forward must have been bg_render_forward_depth (out_depth is its output): otherwise BG_ERR_INVALID
+ * with v_combined and v_z untouched.  The state stays valid until the next forward on the context, of either kind.
+ * bg_project_backward_depth is bg_project_backward followed by v_transforms[gid, 0:3] += v_z[cgid] * R[2,:]
+ * (R = the view rotation, R[2,:] = viewmat[2], viewmat[5], viewmat[8]); Gaussians with v_z == 0 keep
+ * bg_project_backward's output bits. */
+int32_t bg_render_forward_depth(BgContext *ctx, void *stream, const BgCamera *cam, uint32_t w, uint32_t h,
+                                uint32_t n, uint32_t k, const float *transforms, const float *sh,
+                                const float *raw_opac, int32_t mip, const float *bg, int32_t pass,
+                                float *out_img /*[h,w,4]*/, float *out_depth /*[h,w]*/, float *visible,
+                                float *max_radius, BgRenderState *state_out);
+int32_t bg_rasterize_backward_depth(BgContext *ctx, void *stream, const BgRenderState *state, const float *out_img,
+                                    const float *out_depth, const float *v_output, const float *v_depth /*[h,w]*/,
+                                    const float *bg, int32_t smooth_cutoff, float *v_combined,
+                                    uint32_t v_combined_rows, float *v_z /*[v_combined_rows]*/);
+int32_t bg_project_backward_depth(BgContext *ctx, void *stream, const BgCamera *cam, const BgRenderState *state,
+                                  const float *transforms, const float *sh, const float *raw_opac,
+                                  const float *v_combined, const float *v_z, float *v_transforms, float *v_sh,
+                                  float *v_raw_opac, float *v_refine);
 
 /* Measurement aid (not a reference operator): counters of the blend loop for the state of this context's last
  * BG_PASS_BACKWARD forward.  out4 (host): [0] warp-splat iterations of the backward walk (64 pixel-splat pairs each),

@@ -7,6 +7,8 @@
 //   Context                     <- one per logical task, like burn's per-thread stream (brush-async/src/lib.rs:1-17)
 //   render                      <- SplatOps::render            brush-render/src/lib.rs:54-77, render.rs:37-315
 //   rasterize_bwd / project_bwd <- SplatBwdOps                 brush-render/src/bwd/burn_glue.rs:62-92
+//   render_depth, rasterize_bwd_depth, project_bwd_depth
+//                               <- differentiable per-pixel depth (DESIGN.md section 4.6; no reference operator)
 //   radix_argsort / prefix_sum  <- brush-sort/src/lib.rs:16, brush-prefix-sum/src/lib.rs:11
 //   image_loss_forward/backward <- LossOps                     brush-loss/src/lib.rs:718-733
 //   AdamScaled                  <- brush-train/src/adam_scaled.rs:64-165
@@ -253,6 +255,7 @@ struct RenderOutput {                       // render_aux.rs:16-68
     DeviceBuffer<float> out_img_f32;        // [h,w,4] when pass != Forward
     DeviceBuffer<uint32_t> out_img_packed;  // [h,w] rgba8 when pass == Forward
     DeviceBuffer<float> visible, max_radius;   // [n]
+    DeviceBuffer<float> out_depth;          // [h,w] accumulated depth sum_i vis_i z_i (render_depth only)
     BgRenderState state{};                  // device pointers into the context arena, valid until the next render
     BgCamera uniforms{};
     uint32_t w = 0, h = 0;
@@ -303,6 +306,52 @@ inline SplatGrads project_bwd(Context &ctx, cudaStream_t stream, const RenderOut
     check(bg_project_backward(ctx.handle(), stream, &out.uniforms, &out.state, transforms, sh_coeffs, raw_opacities, v_combined,
                               g.v_transforms.data(), g.v_coeffs.data(), g.v_raw_opac.data(), g.v_refine_weight.data()),
           "SplatBwdOps::project_bwd");
+    return g;
+}
+
+// render with the accumulated depth out_depth [h,w] (bg_render_forward_depth): pass Backward or BackwardSmoothCutoff.
+// The expected depth is out_depth / alpha (out_img_f32[..., 3]).
+inline RenderOutput render_depth(Context &ctx, cudaStream_t stream, const Camera &camera, uint32_t img_w, uint32_t img_h,
+                                 const float *transforms, const float *sh_coeffs, const float *raw_opacities, uint32_t n,
+                                 uint32_t k, SplatRenderMode mode, const float background[3], RasterPass pass) {
+    RenderOutput out;
+    out.w = img_w; out.h = img_h;
+    out.uniforms = make_uniforms(camera, img_w, img_h);
+    out.out_img_f32 = DeviceBuffer<float>((size_t)img_w * img_h * 4);
+    out.out_depth = DeviceBuffer<float>((size_t)img_w * img_h);
+    out.visible = DeviceBuffer<float>(n);
+    out.max_radius = DeviceBuffer<float>(n);
+    check(bg_render_forward_depth(ctx.handle(), stream, &out.uniforms, img_w, img_h, n, k, transforms, sh_coeffs,
+                                  raw_opacities, mode == SplatRenderMode::Mip, background, (int32_t)pass,
+                                  out.out_img_f32.data(), out.out_depth.data(), out.visible.data(), out.max_radius.data(),
+                                  &out.state),
+          "render_depth");
+    return out;
+}
+
+// adjoint of render_depth with the upstream gradients v_output [h,w,4] and v_depth [h,w]:
+// returns {v_combined [n,10], v_z [n]} (compact-id order, zero-filled by the callee)
+inline std::pair<DeviceBuffer<float>, DeviceBuffer<float>> rasterize_bwd_depth(Context &ctx, cudaStream_t stream,
+                                                                               const RenderOutput &out, const float *v_output,
+                                                                               const float *v_depth, const float background[3],
+                                                                               bool smooth_cutoff) {
+    DeviceBuffer<float> v_combined((size_t)out.state.n * BG_VCOMBINED_STRIDE), v_z(out.state.n);
+    check(bg_rasterize_backward_depth(ctx.handle(), stream, &out.state, out.out_img_f32.data(), out.out_depth.data(), v_output,
+                                      v_depth, background, smooth_cutoff, v_combined.data(), out.state.n, v_z.data()),
+          "rasterize_bwd_depth");
+    return {std::move(v_combined), std::move(v_z)};
+}
+
+// project_bwd plus the depth chain v_transforms[:, 0:3] += v_z * R[2,:]
+inline SplatGrads project_bwd_depth(Context &ctx, cudaStream_t stream, const RenderOutput &out, const float *transforms,
+                                    const float *sh_coeffs, const float *raw_opacities, const float *v_combined,
+                                    const float *v_z) {
+    const size_t n = out.state.n, k = out.state.k;
+    SplatGrads g{DeviceBuffer<float>(n * 10), DeviceBuffer<float>(n * k * 3), DeviceBuffer<float>(n), DeviceBuffer<float>(n)};
+    check(bg_project_backward_depth(ctx.handle(), stream, &out.uniforms, &out.state, transforms, sh_coeffs, raw_opacities,
+                                    v_combined, v_z, g.v_transforms.data(), g.v_coeffs.data(), g.v_raw_opac.data(),
+                                    g.v_refine_weight.data()),
+          "project_bwd_depth");
     return g;
 }
 
