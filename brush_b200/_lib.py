@@ -16,7 +16,7 @@ BG_OK, BG_ERR_NULL, BG_ERR_INVALID, BG_ERR_CUDA, BG_ERR_CAPACITY, BG_ERR_UNSUPPO
 PASS_FORWARD, PASS_BACKWARD, PASS_BACKWARD_SMOOTH = 0, 1, 2
 PROJECTED_STRIDE = 16
 VCOMBINED_STRIDE = 10
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 _STATUS_NAMES = {1: "BG_ERR_NULL", 2: "BG_ERR_INVALID", 3: "BG_ERR_CUDA", 4: "BG_ERR_CAPACITY", 5: "BG_ERR_UNSUPPORTED"}
 
@@ -80,6 +80,15 @@ class BgTrainStepArgs(C.Structure):
         ("workspace_bytes", C.c_uint64),
         ("loss_out", C.c_void_p),
         ("state_out", BgRenderState),
+    ]
+
+
+class BgDepthSupervision(C.Structure):
+    _fields_ = [
+        ("target", C.c_void_p),
+        ("weight", C.c_float),
+        ("valid_count", C.c_uint32),
+        ("depth_loss_out", C.c_void_p),
     ]
 
 
@@ -191,6 +200,10 @@ SIGNATURES = {
     "bg_normal_noise": (_I32, [_P, _P, C.c_uint64, C.c_uint64, C.c_uint64, _P]),
     "bg_train_step_workspace_bytes": (C.c_uint64, [_U32, _U32, _U32, _U32]),
     "bg_train_step": (_I32, [_P, _P, C.POINTER(BgTrainStepArgs)]),
+    "bg_depth_loss_num_partials": (_U32, [_U32, _U32]),
+    "bg_depth_loss_fused": (_I32, [_P, _P, _P, _P, _P, _U32, _U32, _F, _P, _P, _P]),
+    "bg_train_step_depth_workspace_bytes": (_U64, [_U32, _U32, _U32, _U32]),
+    "bg_train_step_depth": (_I32, [_P, _P, C.POINTER(BgTrainStepArgs), C.POINTER(BgDepthSupervision)]),
     "bg_train_update": (_I32, [_P, _P, C.POINTER(BgTrainUpdateArgs)]),
     "bg_dp_unique_id": (_I32, [_P]),
     "bg_dp_comm_create": (_I32, [_P, _P, _I32, _I32, C.POINTER(_P)]),

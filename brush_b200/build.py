@@ -34,6 +34,7 @@ SOURCES = {
     "dp.cu": [],
     "refine.cu": ["-fmad=false"],
     "lod.cu": ["-fmad=false"],
+    "depth_loss.cu": ["-fmad=false"],
 }
 
 

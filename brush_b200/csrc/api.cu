@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstdint>
 #include <cstring>
@@ -77,6 +78,11 @@ cudaError_t launch_pup_log_det(cudaStream_t, uint32_t, const float *, float *);
 cudaError_t launch_decimate_keys(cudaStream_t, uint32_t, const float *, uint32_t *, uint32_t *);
 cudaError_t launch_decimate_gather(cudaStream_t, uint32_t, uint32_t, const uint32_t *, const float *, const float *,
                                    const float *, const float *, float *, float *, float *, float *);
+// depth_loss.cu
+uint32_t depth_loss_num_partials(uint32_t, uint32_t);
+cudaError_t launch_depth_loss_fused(cudaStream_t, const float *, const float *, const float *, uint32_t, uint32_t, float, float *,
+                                    float *, float *);
+cudaError_t launch_depth_loss_reduce(cudaStream_t, const float *, uint32_t, float, float *, float *);
 }  // namespace bg
 
 using namespace bg;
@@ -580,6 +586,27 @@ extern "C" int32_t bg_image_loss_fused(BgContext *c, void *stream, const float *
     return BG_OK;
 }
 
+extern "C" uint32_t bg_depth_loss_num_partials(uint32_t h, uint32_t w) { return depth_loss_num_partials(h, w); }
+
+extern "C" int32_t bg_depth_loss_fused(BgContext *c, void *stream, const float *out_img, const float *depth,
+                                       const float *target, uint32_t h, uint32_t w, float chain, float *v_output,
+                                       float *v_depth, float *partials) {
+    if (!c || !out_img || !depth || !target || !v_output || !v_depth || !partials) return BG_ERR_NULL;
+    if (h == 0 || w == 0) { set_err("bg_depth_loss_fused: empty image", cudaSuccess); return BG_ERR_INVALID; }
+    if (!(chain >= 0.0f) || !std::isfinite(chain)) { set_err("bg_depth_loss_fused: chain must be finite and >= 0", cudaSuccess); return BG_ERR_INVALID; }
+    if ((((uintptr_t)out_img) | ((uintptr_t)v_output)) & 15u) {
+        set_err("bg_depth_loss_fused: out_img and v_output must be 16-byte aligned (128-bit pixel access)", cudaSuccess);
+        return BG_ERR_INVALID;
+    }
+    if ((((uintptr_t)depth) | ((uintptr_t)target) | ((uintptr_t)v_depth) | ((uintptr_t)partials)) & 3u) {
+        set_err("bg_depth_loss_fused: depth, target, v_depth and partials must be 4-byte aligned", cudaSuccess);
+        return BG_ERR_INVALID;
+    }
+    BG_CUDA(cudaSetDevice(c->device));
+    BG_CUDA(launch_depth_loss_fused((cudaStream_t)stream, out_img, depth, target, h, w, chain, v_output, v_depth, partials));
+    return BG_OK;
+}
+
 // compiler-rt __powisf2, what Rust's f32::powi lowers to (adam_scaled.rs:135-142)
 static float powi_f32(float a, int b) {
     const bool recip = b < 0;
@@ -741,6 +768,61 @@ TrainWs carve_train_ws(void *base, uint32_t n, uint32_t k, uint32_t w, uint32_t 
     ws.bytes = off;
     return ws;
 }
+
+// the depth step's extra scratch, behind the largest plain-step workspace
+struct DepthWs {
+    float *depth, *v_depth, *v_z, *partials;
+    uint64_t bytes;
+};
+DepthWs carve_depth_ws(void *base, uint32_t n, uint32_t k, uint32_t w, uint32_t h) {
+    uint64_t off = carve_train_ws(nullptr, n, k, w, h, 4).bytes;
+    auto take = [&](uint64_t floats) {
+        float *p = base ? reinterpret_cast<float *>(static_cast<char *>(base) + off) : nullptr;
+        off += (floats * 4 + 255) / 256 * 256;
+        return p;
+    };
+    DepthWs ws;
+    const uint64_t px = (uint64_t)w * h;
+    ws.depth = take(px);
+    ws.v_depth = take(px);
+    ws.v_z = take(std::max(n, 1u));
+    ws.partials = take(depth_loss_num_partials(h, w));
+    ws.bytes = off;
+    return ws;
+}
+
+// argument checks shared by bg_train_step and bg_train_step_depth
+int32_t check_train_args(const BgTrainStepArgs *a, const char *who) {
+    if (!a->transforms || !a->sh || !a->raw_opac || !a->m_t || !a->v_t || !a->m_sh || !a->v_sh || !a->m_o || !a->v_o ||
+        !a->refine_norm || !a->vis_weight || !a->max_screen || !a->gt_packed || !a->workspace || !a->loss_out)
+        return BG_ERR_NULL;
+    char m[160];
+    auto invalid = [&](const char *what) {
+        snprintf(m, sizeof(m), "%s: %s", who, what);
+        set_err(m, cudaSuccess);
+        return BG_ERR_INVALID;
+    };
+    if (a->step < 1) return invalid("step is 1-based");
+    if (a->channels != 3 && a->channels != 4) return invalid("channels must be 3 or 4");
+    if ((uintptr_t)a->workspace % 256) return invalid("workspace must be 256-byte aligned");
+    return BG_OK;
+}
+
+// optimiser, refine statistics, mean noise (train.rs:280-416): one pass over the Gaussians
+int32_t run_train_update(BgContext *c, void *stream, const BgTrainStepArgs *a, const TrainWs &ws) {
+    BgTrainUpdateArgs up;
+    memset(&up, 0, sizeof(up));
+    up.n = a->n; up.k = a->k;
+    up.transforms = a->transforms; up.sh = a->sh; up.raw_opac = a->raw_opac;
+    up.m_t = a->m_t; up.v_t = a->v_t; up.m_sh = a->m_sh; up.v_sh = a->v_sh; up.m_o = a->m_o; up.v_o = a->v_o;
+    up.refine_norm = a->refine_norm; up.vis_weight = a->vis_weight; up.max_screen = a->max_screen;
+    up.v_transforms = ws.v_t; up.v_sh_grad = ws.v_sh; up.v_raw_opac = ws.v_o;
+    up.v_refine = ws.v_r; up.visible = ws.visible; up.max_radius = ws.max_radius;
+    up.lr_mean = a->lr_mean; up.lr_rotation = a->lr_rotation; up.lr_scale = a->lr_scale; up.lr_coeffs_dc = a->lr_coeffs_dc;
+    up.lr_coeffs_sh_scale = a->lr_coeffs_sh_scale; up.lr_opac = a->lr_opac;
+    up.noise_scale = a->noise_scale; up.median_scale = a->median_scale; up.seed = a->seed; up.step = a->step;
+    return bg_train_update(c, stream, &up);
+}
 }  // namespace
 
 extern "C" uint64_t bg_train_step_workspace_bytes(uint32_t n, uint32_t k, uint32_t w, uint32_t h) {
@@ -749,12 +831,7 @@ extern "C" uint64_t bg_train_step_workspace_bytes(uint32_t n, uint32_t k, uint32
 
 extern "C" int32_t bg_train_step(BgContext *c, void *stream, BgTrainStepArgs *a) {
     if (!c || !a) return BG_ERR_NULL;
-    if (!a->transforms || !a->sh || !a->raw_opac || !a->m_t || !a->v_t || !a->m_sh || !a->v_sh || !a->m_o || !a->v_o ||
-        !a->refine_norm || !a->vis_weight || !a->max_screen || !a->gt_packed || !a->workspace || !a->loss_out)
-        return BG_ERR_NULL;
-    if (a->step < 1) { set_err("bg_train_step: step is 1-based", cudaSuccess); return BG_ERR_INVALID; }
-    if (a->channels != 3 && a->channels != 4) { set_err("bg_train_step: channels must be 3 or 4", cudaSuccess); return BG_ERR_INVALID; }
-    if ((uintptr_t)a->workspace % 256) { set_err("bg_train_step: workspace must be 256-byte aligned", cudaSuccess); return BG_ERR_INVALID; }
+    if (int32_t r = check_train_args(a, "bg_train_step"); r != BG_OK) return r;
     const uint32_t n = a->n, k = a->k, w = a->w, h = a->h;
     const TrainWs ws = carve_train_ws(a->workspace, n, k, w, h, a->channels);
     if (ws.bytes > a->workspace_bytes) { set_err("bg_train_step: workspace too small (bg_train_step_workspace_bytes)", cudaSuccess); return BG_ERR_CAPACITY; }
@@ -778,19 +855,61 @@ extern "C" int32_t bg_train_step(BgContext *c, void *stream, BgTrainStepArgs *a)
     if (r != BG_OK) return r;
     r = bg_project_backward(c, stream, &a->cam, &a->state_out, a->transforms, a->sh, a->raw_opac, ws.v_combined, ws.v_t, ws.v_sh, ws.v_o, ws.v_r);
     if (r != BG_OK) return r;
-    // optimiser, refine statistics, mean noise (train.rs:280-416): one pass over the Gaussians
-    BgTrainUpdateArgs up;
-    memset(&up, 0, sizeof(up));
-    up.n = n; up.k = k;
-    up.transforms = a->transforms; up.sh = a->sh; up.raw_opac = a->raw_opac;
-    up.m_t = a->m_t; up.v_t = a->v_t; up.m_sh = a->m_sh; up.v_sh = a->v_sh; up.m_o = a->m_o; up.v_o = a->v_o;
-    up.refine_norm = a->refine_norm; up.vis_weight = a->vis_weight; up.max_screen = a->max_screen;
-    up.v_transforms = ws.v_t; up.v_sh_grad = ws.v_sh; up.v_raw_opac = ws.v_o;
-    up.v_refine = ws.v_r; up.visible = ws.visible; up.max_radius = ws.max_radius;
-    up.lr_mean = a->lr_mean; up.lr_rotation = a->lr_rotation; up.lr_scale = a->lr_scale; up.lr_coeffs_dc = a->lr_coeffs_dc;
-    up.lr_coeffs_sh_scale = a->lr_coeffs_sh_scale; up.lr_opac = a->lr_opac;
-    up.noise_scale = a->noise_scale; up.median_scale = a->median_scale; up.seed = a->seed; up.step = a->step;
-    return bg_train_update(c, stream, &up);
+    return run_train_update(c, stream, a, ws);
+}
+
+// ---- bg_train_step_depth: bg_train_step with the depth-supervision term of DESIGN.md section 4.7
+extern "C" uint64_t bg_train_step_depth_workspace_bytes(uint32_t n, uint32_t k, uint32_t w, uint32_t h) {
+    return carve_depth_ws(nullptr, n, k, w, h).bytes;
+}
+
+extern "C" int32_t bg_train_step_depth(BgContext *c, void *stream, BgTrainStepArgs *a, const BgDepthSupervision *d) {
+    if (!c || !a || !d || !d->depth_loss_out) return BG_ERR_NULL;
+    if (!(d->weight >= 0.0f) || !std::isfinite(d->weight)) {
+        set_err("bg_train_step_depth: weight must be finite and >= 0", cudaSuccess);
+        return BG_ERR_INVALID;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    if (d->weight == 0.0f || d->valid_count == 0) {
+        // no term (target may be null): the plain step, launch for launch, and a zero depth loss
+        const int32_t r = bg_train_step(c, stream, a);
+        if (r != BG_OK) return r;
+        BG_CUDA(cudaMemsetAsync(d->depth_loss_out, 0, sizeof(float), s));
+        return BG_OK;
+    }
+    if (!d->target) return BG_ERR_NULL;
+    if (int32_t r = check_train_args(a, "bg_train_step_depth"); r != BG_OK) return r;
+    const uint32_t n = a->n, k = a->k, w = a->w, h = a->h;
+    const TrainWs ws = carve_train_ws(a->workspace, n, k, w, h, a->channels);
+    const DepthWs dws = carve_depth_ws(a->workspace, n, k, w, h);
+    if (dws.bytes > a->workspace_bytes) {
+        set_err("bg_train_step_depth: workspace too small (bg_train_step_depth_workspace_bytes)", cudaSuccess);
+        return BG_ERR_CAPACITY;
+    }
+    BG_CUDA(cudaSetDevice(c->device));
+    int32_t r;
+    r = bg_render_forward_depth(c, stream, &a->cam, w, h, n, k, a->transforms, a->sh, a->raw_opac, a->mip, a->background,
+                                BG_PASS_BACKWARD, ws.out_img, dws.depth, ws.visible, ws.max_radius, &a->state_out);
+    if (r != BG_OK) return r;
+    const float npx = (float)w * (float)h;
+    float chain[4] = {1.0f / (3.0f * npx), 1.0f / (3.0f * npx), 1.0f / (3.0f * npx), a->channels == 4 ? a->alpha_weight / npx : 0.0f};
+    BG_CUDA(cudaMemsetAsync(ws.v_output, 0, (size_t)w * h * 4 * sizeof(float), s));
+    r = bg_image_loss_fused(c, stream, ws.out_img, a->gt_packed, a->channels, h, w, 1, (int64_t)w * 4, 4, a->l1_weight, a->ssim_weight,
+                            a->has_composite_bg ? a->composite_bg : nullptr, a->mask, chain, ws.v_output, ws.partials);
+    if (r != BG_OK) return r;
+    BG_CUDA(launch_loss_reduce(s, ws.partials, a->channels, bg_image_loss_num_partials(a->channels, h, w) / a->channels, chain, a->loss_out));
+    // depth term: v_depth, v_output[...,3] += dL/da, L_d -> depth_loss_out and added to loss_out
+    const float dchain = d->weight / (float)d->valid_count;
+    r = bg_depth_loss_fused(c, stream, ws.out_img, dws.depth, d->target, h, w, dchain, ws.v_output, dws.v_depth, dws.partials);
+    if (r != BG_OK) return r;
+    BG_CUDA(launch_depth_loss_reduce(s, dws.partials, depth_loss_num_partials(h, w), dchain, d->depth_loss_out, a->loss_out));
+    r = bg_rasterize_backward_depth(c, stream, &a->state_out, ws.out_img, dws.depth, ws.v_output, dws.v_depth, a->background, 0,
+                                    ws.v_combined, n, dws.v_z);
+    if (r != BG_OK) return r;
+    r = bg_project_backward_depth(c, stream, &a->cam, &a->state_out, a->transforms, a->sh, a->raw_opac, ws.v_combined, dws.v_z,
+                                  ws.v_t, ws.v_sh, ws.v_o, ws.v_r);
+    if (r != BG_OK) return r;
+    return run_train_update(c, stream, a, ws);
 }
 
 // ---- view-sharded data parallelism (dp.cu): communicator, exchange, the multi-view step

@@ -13,6 +13,8 @@
   load_realitycapture             <- formats/realitycapture.rs (camera csv: 35 mm-film intrinsics, heading / pitch / roll)
   find_image_by_name, find_mask_path, split_eval_every, opengl_c2w_to_pose <- formats/mod.rs:112-189
   SceneView.load_image            <- load_image.rs:59-123 (decode, mask file -> alpha channel, resolution cap)
+  SceneView.load_depth, find_depth_path <- per-view depth maps for depth supervision (DESIGN.md section 4.7; nerfstudio's
+                                      `depth_file_path`, COLMAP `depths/`); no reference counterpart
   COLMAP text / binary grammar    <- colmap-reader/src/lib.rs (cameras / images / points3D, .txt and .bin)
   SceneLoader                     <- scene_loader.rs:13-170 (loader threads, bounded prefetch queue, packed-batch cache)
 
@@ -264,6 +266,57 @@ def find_mask_path(files: Sequence[str], path: str) -> Optional[str]:
     return None
 
 
+def find_depth_path(files: Sequence[str], path: str) -> Optional[str]:
+    """The depth map of a COLMAP image: `<stem>.png` or `<stem>.npy` (any case) under a directory called `depths` (any
+    case), whose sub-directories below `depths/` must be the tail of the image's own directory, as find_mask_path requires
+    of masks: depths/foo/img.png matches images/foo/img.jpg.  First match in `files` order."""
+    norm = lambda q: [c for c in q.replace("\\", "/").split("/") if c not in ("", ".")]
+    comps = norm(path)
+    name = comps[-1].lower()
+    stem = name.rsplit(".", 1)[0] if "." in name[1:] else name
+    wanted = {stem + ".png", stem + ".npy"}
+    parent = comps[:-1]
+    for cand in files:
+        cc = norm(cand)
+        if not cc or cc[-1].lower() not in wanted:
+            continue
+        idx = next((i for i, c in enumerate(cc) if c.lower() == "depths"), None)
+        if idx is None:
+            continue
+        sub = cc[idx + 1:-1]
+        if len(sub) <= len(parent) and (not sub or parent[len(parent) - len(sub):] == sub):
+            return cand
+    return None
+
+
+def decode_depth(path: str) -> np.ndarray:
+    """A single-channel depth file -> f32 [H,W] in file units: `.npy` (2-D or [H,W,1]) or a PNG / TIFF in PIL mode
+    I;16, I, F or L.  Anything with more than one channel is a ValueError."""
+    if path.lower().endswith(".npy"):
+        a = np.load(path, allow_pickle=False)
+        if a.ndim == 3 and a.shape[2] == 1:
+            a = a[..., 0]
+        if a.ndim != 2:
+            raise ValueError(f"depth map {path}: expected [H,W] or [H,W,1], got shape {a.shape}")
+        return np.asarray(a, np.float32)
+    from PIL import Image
+    with Image.open(path) as im:
+        if im.mode not in ("I;16", "I;16B", "I;16L", "I", "F", "L"):
+            raise ValueError(f"depth map {path}: expected a single-channel image (I;16, I, F or L), got mode {im.mode}")
+        return np.asarray(im).astype(np.float32)
+
+
+def resize_nearest(a: np.ndarray, w: int, h: int) -> np.ndarray:
+    """Nearest-neighbour resize of [H,W] to [h,w] with pixel centres aligned: source index floor((i + 0.5) * src / dst).
+    Never blends values, so invalid zeros stay apart from valid depths."""
+    sh, sw = a.shape
+    if (sh, sw) == (h, w):
+        return a
+    ys = np.minimum(((np.arange(h) + 0.5) * sh / h).astype(np.int64), sh - 1)
+    xs = np.minimum(((np.arange(w) + 0.5) * sw / w).astype(np.int64), sw - 1)
+    return a[ys[:, None], xs[None, :]]
+
+
 def scaled_image_size(w: int, h: int, scale: float, max_resolution: Optional[int] = None) -> Tuple[int, int]:
     """LoadImage::output_scale + load (load_image.rs:115-131), in f32: factor = min(cap * scale, 1) with
     cap = max_res / max(w, h, max_res) (1 without a cap); the size is trunc(max(side * factor, 1)), unchanged when the
@@ -282,6 +335,8 @@ class SceneView:
     image_path: str
     mask_path: Optional[str] = None      # load_image.rs:15: a separate mask image that becomes the alpha channel
     invert_mask: bool = False            # config.rs:46-48: white means "ignore this pixel"
+    depth_path: Optional[str] = None     # a per-view depth map (DESIGN.md section 4.7)
+    depth_scale: float = 1.0             # file units -> scene units (the dataset's depth_unit_scale_factor)
 
     def default_alpha_mode(self) -> str:
         """LoadImage::new (load_image.rs:41-47): a view with a mask file is Masked, anything else Transparent, unless the
@@ -323,6 +378,29 @@ class SceneView:
             im = im.resize((max(1, round(im.size[0] * s)), max(1, round(im.size[1] * s))), Image.LANCZOS)
         return np.asarray(im, np.uint8)
 
+    def image_size(self, max_resolution: Optional[int] = None, scale: float = 1.0) -> Tuple[int, int]:
+        """(w, h) of load_image(max_resolution, scale), from the image header alone."""
+        from PIL import Image
+        with Image.open(self.image_path) as im:
+            w, h = im.size
+        if scale < 1.0:
+            return scaled_image_size(w, h, scale, max_resolution)
+        if max_resolution and max(w, h) > max_resolution:
+            s = max_resolution / max(w, h)
+            return max(1, round(w * s)), max(1, round(h * s))
+        return w, h
+
+    def load_depth(self, max_resolution: Optional[int] = None, scale: float = 1.0) -> Optional[np.ndarray]:
+        """The view's depth target as f32 [H,W] in scene units, at exactly the size load_image(max_resolution, scale)
+        returns: decoded (decode_depth), multiplied by depth_scale, nearest-resized; non-finite or <= 0 values become 0
+        (no measurement).  None when the view has no depth map."""
+        if self.depth_path is None:
+            return None
+        d = decode_depth(self.depth_path) * np.float32(self.depth_scale)
+        w, h = self.image_size(max_resolution, scale)
+        d = resize_nearest(d, w, h)
+        return np.ascontiguousarray(np.where(np.isfinite(d) & (d > 0), d, np.float32(0.0)), np.float32)
+
 
 @dataclass
 class DatasetLoadResult:
@@ -344,9 +422,11 @@ def list_files(root: str) -> List[str]:
 def find_image_by_name(files: Sequence[str], name: str) -> Optional[str]:
     """formats/mod.rs:112-120: colmap stores a bare (or sub-directory) file name; the image is the lexicographically first
     file whose path ends with it on a component boundary (case-insensitive, like the vfs keys), never one under a
-    `masks` directory -- an image must not resolve to its own mask."""
+    `masks` directory -- an image must not resolve to its own mask -- nor under a `depths` directory (any case), where its
+    depth map may carry the image's own file name (find_depth_path)."""
     key = "/" + name.replace("\\", "/").lower().lstrip("/")
-    hits = [f for f in files if ("/" + f.lower()).endswith(key) and "masks" not in f.split("/")[:-1]]
+    hits = [f for f in files if ("/" + f.lower()).endswith(key) and "masks" not in f.split("/")[:-1]
+            and not any(c.lower() == "depths" for c in f.split("/")[:-1])]
     return min(hits) if hits else None
 
 
@@ -361,9 +441,10 @@ def _find(root: str, name: str) -> Optional[str]:
 
 def load_colmap(root: str, subsample_frames: Optional[int] = None, max_frames: Optional[int] = None,
                 eval_split_every: Optional[int] = None, subsample_points: Optional[int] = None,
-                invert_masks: bool = False) -> DatasetLoadResult:
+                invert_masks: bool = False, depth_unit_scale_factor: float = 1e-3) -> DatasetLoadResult:
     """Text or binary COLMAP model (cameras.{txt,bin} decides; images / points3D are taken from the same directory).
-    Views whose image has a counterpart under a `masks/` directory carry it as their alpha channel (colmap.rs:194-218)."""
+    Views whose image has a counterpart under a `masks/` directory carry it as their alpha channel (colmap.rs:194-218),
+    views with a `depths/<stem>.png|.npy` (find_depth_path) a depth map in units of depth_unit_scale_factor."""
     cam_path = _find(root, "cameras.bin") or _find(root, "cameras.txt")
     if cam_path is None:
         raise FileNotFoundError("no cameras.txt / cameras.bin under " + root)
@@ -377,7 +458,7 @@ def load_colmap(root: str, subsample_frames: Optional[int] = None, max_frames: O
         infos = read_images_text(open(os.path.join(sparse, "images.txt")).read())
     infos = sorted(infos, key=lambda i: i.name)
     views, warnings = [], []
-    files = mask_files = None                              # the dataset's file list / mask candidates, listed once
+    files = mask_files = depth_files = None                # the dataset's file list / mask / depth candidates, listed once
     picked = infos[::max(int(subsample_frames or 1), 1)]
     if max_frames is not None:
         picked = picked[:max_frames]
@@ -399,7 +480,11 @@ def load_colmap(root: str, subsample_frames: Optional[int] = None, max_frames: O
             mask_files = [f for f in files if any(c.lower() == "masks" for c in f.split("/")[:-1])]
         mask = find_mask_path(mask_files, rel) if mask_files else None
         mask = os.path.join(root, mask) if mask is not None else None
-        views.append(SceneView(camera, path, mask, bool(invert_masks) and mask is not None))
+        if depth_files is None:
+            depth_files = [f for f in files if any(c.lower() == "depths" for c in f.split("/")[:-1])]
+        depth = find_depth_path(depth_files, rel) if depth_files else None
+        views.append(SceneView(camera, path, mask, bool(invert_masks) and mask is not None,
+                               os.path.join(root, depth) if depth is not None else None, float(depth_unit_scale_factor)))
     train, ev = split_eval_every(views, eval_split_every)
     init = None
     pts_txt, pts_bin = os.path.join(sparse, "points3D.txt"), os.path.join(sparse, "points3D.bin")
@@ -471,8 +556,23 @@ def _nerfstudio_camera_model(name, k1, k2, k3, k4, p1, p2):
     raise ValueError(f"Error decoding camera parameters: Unsupported nerfstudio camera_model `{name}`")
 
 
+def _resolve_frame_file(fp: str, base: str, root: str, lower: dict) -> Optional[str]:
+    """A frame's file reference -> the dataset file it names (relative to root), or None."""
+    if os.path.isabs(fp):        # absolute references are resolved inside the dataset directory only (brush-vfs lib.rs:313-325)
+        fp_rel = os.path.relpath(fp, os.path.abspath(root))
+        rel = fp_rel.replace(os.sep, "/") if not fp_rel.startswith("..") else "\0outside"
+    else:
+        rel = os.path.normpath(os.path.join(base, fp)).replace(os.sep, "/")
+    hit = lower.get(rel.lower())
+    if hit is None and not os.path.splitext(rel)[1]:
+        # "Assume png's by default if no extension is specified" (nerfstudio.rs:183-186; the reference tests existence
+        # before adding the extension, which would skip every such frame -- its stated intent is followed here)
+        hit = lower.get((rel + ".png").lower())
+    return hit
+
+
 def _read_transforms_file(scene: dict, transforms_rel: str, root: str, files: Sequence[str], subsample_frames, max_frames,
-                          invert_masks: bool, warnings: List[str]) -> List[SceneView]:
+                          invert_masks: bool, warnings: List[str], depth_unit_scale_factor: float = 1e-3) -> List[SceneView]:
     """read_transforms_file (nerfstudio.rs:142-268).  Per-frame values override the file-level ones."""
     lower = {f.lower(): f for f in files}
     mask_files = [f for f in files if any(c.lower() == "masks" for c in f.split("/")[:-1])]
@@ -487,17 +587,7 @@ def _read_transforms_file(scene: dict, transforms_rel: str, root: str, files: Se
             raise ValueError(f"Error when decoding format: frame '{fr['file_path']}' has a {len(flat)}-element transform_matrix, "
                              "expected a 4x4 (16 elements)")
         pos, rot = opengl_c2w_to_pose(np.array(flat, np.float32).reshape(4, 4))
-        fp = fr["file_path"]
-        if os.path.isabs(fp):        # absolute references are resolved inside the dataset directory only (brush-vfs lib.rs:313-325)
-            fp_rel = os.path.relpath(fp, os.path.abspath(root))
-            rel = fp_rel.replace(os.sep, "/") if not fp_rel.startswith("..") else "\0outside"
-        else:
-            rel = os.path.normpath(os.path.join(base, fp)).replace(os.sep, "/")
-        hit = lower.get(rel.lower())
-        if hit is None and not os.path.splitext(rel)[1]:
-            # "Assume png's by default if no extension is specified" (nerfstudio.rs:183-186; the reference tests existence
-            # before adding the extension, which would skip every such frame -- its stated intent is followed here)
-            hit = lower.get((rel + ".png").lower())
+        hit = _resolve_frame_file(fr["file_path"], base, root, lower)
         if hit is None:
             warnings.append(f"Skipped '{fr['file_path']}': image file not found")
             continue
@@ -532,17 +622,25 @@ def _read_transforms_file(scene: dict, transforms_rel: str, root: str, files: Se
             warnings.append(f"Skipped '{fr['file_path']}': camera contains nan or inf values")
             continue
         mask = find_mask_path(mask_files, hit) if mask_files else None
+        depth = None
+        if fr.get("depth_file_path"):                    # resolved exactly like file_path
+            depth = _resolve_frame_file(fr["depth_file_path"], base, root, lower)
+            if depth is None:
+                warnings.append(f"'{fr['file_path']}': depth file '{fr['depth_file_path']}' not found, the view has no depth")
         views.append(SceneView(camera, os.path.join(root, hit), os.path.join(root, mask) if mask else None,
-                               bool(invert_masks) and mask is not None))
+                               bool(invert_masks) and mask is not None, os.path.join(root, depth) if depth else None,
+                               float(depth_unit_scale_factor)))
     return views
 
 
 def load_nerfstudio(root: str, subsample_frames: Optional[int] = None, max_frames: Optional[int] = None,
                     eval_split_every: Optional[int] = None, subsample_points: Optional[int] = None,
-                    invert_masks: bool = False) -> Optional[DatasetLoadResult]:
+                    invert_masks: bool = False, depth_unit_scale_factor: float = 1e-3) -> Optional[DatasetLoadResult]:
     """nerfstudio.rs:270-388.  None when the directory holds no transforms json (the caller tries the next format).
     The training file is the only json, else `transforms.json`, else `transforms_train.json`; `transforms_val.json` (or
-    `transforms_test.json`) provides the evaluation views, otherwise every eval_split_every-th training view does."""
+    `transforms_test.json`) provides the evaluation views, otherwise every eval_split_every-th training view does.
+    A frame's `depth_file_path` (resolved like `file_path`) is its depth map, in units of depth_unit_scale_factor
+    (nerfstudio's default: millimetres); a missing depth file is a warning and the view keeps no depth."""
     import json
     files = list_files(root)
     jsons = [f for f in files if f.lower().endswith(".json")]
@@ -555,14 +653,15 @@ def load_nerfstudio(root: str, subsample_frames: Optional[int] = None, max_frame
         return None
     warnings: List[str] = []
     scene = json.load(open(os.path.join(root, tpath)))
-    train_all = _read_transforms_file(scene, tpath, root, files, subsample_frames, max_frames, invert_masks, warnings)
+    train_all = _read_transforms_file(scene, tpath, root, files, subsample_frames, max_frames, invert_masks, warnings,
+                                      depth_unit_scale_factor)
     ends = lambda f, name: f.split("/")[-1] == name
     eval_path = next((f for f in jsons if ends(f, "transforms_val.json")), None) or \
         next((f for f in jsons if ends(f, "transforms_test.json")), None)
     val_views = None
     if eval_path is not None:
         val_views = _read_transforms_file(json.load(open(os.path.join(root, eval_path))), eval_path, root, files, subsample_frames,
-                                          max_frames, invert_masks, warnings)
+                                          max_frames, invert_masks, warnings, depth_unit_scale_factor)
     train, ev = [], []
     for i, v in enumerate(train_all):
         if eval_split_every and i % eval_split_every == 0 and val_views is None:   # extra eval images only without a val file
@@ -689,17 +788,17 @@ def load_realitycapture(root: str, subsample_frames: Optional[int] = None, max_f
 
 def load_dataset(root: str, subsample_frames: Optional[int] = None, max_frames: Optional[int] = None,
                  eval_split_every: Optional[int] = None, subsample_points: Optional[int] = None,
-                 invert_masks: bool = False) -> DatasetLoadResult:
+                 invert_masks: bool = False, depth_unit_scale_factor: float = 1e-3) -> DatasetLoadResult:
     """formats/mod.rs:57-110: COLMAP first, then nerfstudio json, then a RealityCapture csv; a dataset without a usable training view is an error; an
     `init.ply` (else the last .ply by name) anywhere in the directory overrides the format's own initial points."""
     args = dict(subsample_frames=subsample_frames, max_frames=max_frames, eval_split_every=eval_split_every,
                 subsample_points=subsample_points, invert_masks=invert_masks)
     if _find(root, "cameras.bin") or _find(root, "cameras.txt"):
-        res = load_colmap(root, **args)
+        res = load_colmap(root, **args, depth_unit_scale_factor=depth_unit_scale_factor)
     else:
-        res = load_nerfstudio(root, **args)
+        res = load_nerfstudio(root, **args, depth_unit_scale_factor=depth_unit_scale_factor)
         if res is None:
-            res = load_realitycapture(root, **args)
+            res = load_realitycapture(root, **args)          # RealityCapture exports carry no depth
         if res is None:
             raise ValueError("Format not recognized: only colmap, nerfstudio json and RealityCapture csv are supported")
     if not res.train:
@@ -752,14 +851,20 @@ class SceneLoader:
         packed, has_alpha = v.load_packed(self.alpha_mode, scale=self.image_scale)
         t = torch.from_numpy(np.ascontiguousarray(packed).view(np.int32))
         nbytes = t.numel() * 4
+        depth, depth_count = None, 0
+        if v.depth_path is not None:                        # the depth target at the image's size, |valid| counted here
+            dm = v.load_depth(scale=self.image_scale)
+            depth, depth_count = torch.from_numpy(dm), int(np.count_nonzero(dm))
+            nbytes += depth.numel() * 4
         with self._lock:
             if self._cache[index] is not None:              # another loader task produced it meanwhile: one buffer per view
                 return self._cache[index]
             admit = self._cache_used + nbytes < self._cache_budget
         if admit and torch.cuda.is_available():
             t = t.pin_memory()      # cached batches are uploaded many times: pin them once
+            depth = depth.pin_memory() if depth is not None else None
         batch = SceneBatch(img_packed=t, camera=v.camera, has_alpha=has_alpha,
-                           masked_alpha=has_alpha and self.alpha_mode == ALPHA_MASKED)
+                           masked_alpha=has_alpha and self.alpha_mode == ALPHA_MASKED, depth=depth, depth_count=depth_count)
         if admit:
             with self._lock:
                 if self._cache[index] is not None:

@@ -178,14 +178,21 @@ def train_loop(ctx, splats, train_views: Sequence, eval_views: Sequence, config,
             on_step(done, stats, refine)
         if eval_views and should_eval_lod(done, level, process.eval_every, total):
             check_overflow()
-            psnr, ssim = [], []
+            psnr, ssim, dm = [], [], []
             for v in eval_views:
                 gt = v.load_image()                        # view.image.load(): a mask file, if any, is the alpha channel
-                s = eval_stats(ctx, splats, v.camera, gt, alpha_mode, render_mip=config.render_mip)
+                gt_depth = v.load_depth() if v.depth_path is not None else None
+                s = eval_stats(ctx, splats, v.camera, gt, alpha_mode, render_mip=config.render_mip, gt_depth=gt_depth)
                 psnr.append(float(s.psnr)); ssim.append(float(s.ssim))
+                if gt_depth is not None:
+                    dm.append((float(s.depth_abs_rel), float(s.depth_rmse), float(s.depth_coverage)))
                 if process.eval_save_to_disk:              # train_stream.rs:543-550
                     s.save_to_disk(os.path.join(process.export_path, f"eval_{done}", f"{v.img_name()}.png"))
-            evals.append({"iter": done, "psnr": float(np.mean(psnr)), "ssim": float(np.mean(ssim)), "splats": splats.num_splats()})
+            rec = {"iter": done, "psnr": float(np.mean(psnr)), "ssim": float(np.mean(ssim)), "splats": splats.num_splats()}
+            if dm:                                         # only when the eval views carry depth (means over those views)
+                for key, col in zip(("depth_abs_rel", "depth_rmse", "depth_coverage"), np.array(dm, np.float64).T):
+                    rec[key] = float(np.mean(col))
+            evals.append(rec)
         if should_export_lod(done, level, process.export_every, total_all, config.lod_levels):
             export(lod_export_name(process.export_name, level, done, steps))
     torch.cuda.synchronize(ctx.device)

@@ -99,6 +99,26 @@ def image_loss_fused(ctx: RenderContext, pred_hwc: torch.Tensor, gt_packed: torc
     return out_hwc, loss
 
 
+def depth_loss_fused(ctx: RenderContext, pred_hwc: torch.Tensor, depth: torch.Tensor, target: torch.Tensor, chain: float,
+                     out_hwc: torch.Tensor, v_depth: Optional[torch.Tensor] = None):
+    """Depth-supervision term (bg_depth_loss_fused, DESIGN.md section 4.7) of a depth render: pred_hwc = out_img [h,w,4],
+    depth = D [h,w], target = t [h,w] (valid where finite and > 0), chain = w_d / |valid pixels|.  ADDS dL/dalpha to
+    out_hwc[...,3] in place on the active pixels and returns (v_depth [h,w], L_d scalar tensor)."""
+    lib = _lib.load()
+    h, w = pred_hwc.shape[0], pred_hwc.shape[1]
+    for t, name, shape in ((pred_hwc, "pred_hwc", (h, w, 4)), (out_hwc, "out_hwc", (h, w, 4)), (depth, "depth", (h, w)),
+                           (target, "target", (h, w))):
+        if t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous() or tuple(t.shape) != shape:
+            raise ValueError(f"{name} must be a contiguous float32 CUDA tensor of shape {shape}")
+    if v_depth is None:
+        v_depth = torch.empty((h, w), dtype=torch.float32, device=pred_hwc.device)
+    partials = torch.empty(int(lib.bg_depth_loss_num_partials(h, w)), dtype=torch.float32, device=pred_hwc.device)
+    _lib.check(lib.bg_depth_loss_fused(ctx.handle, _stream_ptr(ctx.device), pred_hwc.data_ptr(), depth.data_ptr(),
+                                       target.data_ptr(), h, w, float(chain), out_hwc.data_ptr(), v_depth.data_ptr(),
+                                       partials.data_ptr()), "bg_depth_loss_fused")
+    return v_depth, partials.sum() * float(chain)
+
+
 class _ImageLoss(torch.autograd.Function):
     @staticmethod
     def forward(fctx, pred_hwc, gt_packed, ctx, channels, cfg):

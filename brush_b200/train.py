@@ -35,9 +35,9 @@ import torch
 
 from . import _lib
 from .camera import Camera
-from .loss import ImageLossConfig, image_loss_fused
+from .loss import ImageLossConfig, depth_loss_fused, image_loss_fused
 from .render import (PASS_BACKWARD, RenderContext, _stream_ptr, project_bwd, project_bwd_factored, rasterize_bwd,
-                     render_splats, sh_grad_from_views)
+                     rasterize_bwd_depth, render_splats, sh_grad_from_views)
 
 
 @dataclass
@@ -63,6 +63,10 @@ class TrainConfig:
     background_color: Sequence[float] = (0.0, 0.0, 0.0)
     background_noise_strength: float = 0.1
     render_mip: bool = False
+    # depth supervision (DESIGN.md section 4.7): weight of the L1 term on the expected depth of views that carry a depth
+    # map; 0 leaves the step exactly as without it.  Keyword-only, so the positional order of every other field and the
+    # trailing seed + LOD fields stay as they were.
+    depth_loss_weight: float = field(default=0.0, kw_only=True)
     seed: int = 0  # the reference uses an unseeded rand::rng(); a shared seed keeps DP ranks identical
     # LOD baking (config.rs:108-125): after the main run, lod_levels times score, keep lod_decimation_keep % of the splats
     # and retrain lod_refine_steps steps on images scaled by lod_image_scale % per level
@@ -72,6 +76,8 @@ class TrainConfig:
     lod_image_scale: int = 50
 
     def __post_init__(self):
+        if not (math.isfinite(self.depth_loss_weight) and self.depth_loss_weight >= 0.0):
+            raise ValueError(f"depth_loss_weight must be finite and >= 0, got {self.depth_loss_weight}")
         if self.lod_levels < 0:
             raise ValueError("lod_levels must be >= 0")
         for name in ("lod_decimation_keep", "lod_image_scale"):
@@ -143,6 +149,8 @@ class SceneBatch:
     camera: Camera
     has_alpha: bool = False
     masked_alpha: bool = False    # AlphaMode::Masked
+    depth: Optional[torch.Tensor] = None   # [H,W] f32 metric camera-space z target, 0 = no measurement; host (pinned) or device
+    depth_count: int = 0                    # valid pixels of `depth` (finite and > 0), counted on the host
 
     def img_size(self):
         return int(self.img_packed.shape[0]), int(self.img_packed.shape[1])
@@ -220,7 +228,8 @@ def bounds_from_pos_device(ctx: RenderContext, percentile: float, transforms: to
 class TrainStepStats:
     num_visible_event: object
     lr_mean: float
-    loss: torch.Tensor  # lazy device scalar (msg.rs:16-27)
+    loss: torch.Tensor  # lazy device scalar (msg.rs:16-27); image loss + depth loss
+    depth_loss: Optional[torch.Tensor] = None   # the depth term alone (None when the batch carries no depth)
 
 
 class SplatTrainer:
@@ -248,6 +257,8 @@ class SplatTrainer:
         self._dp_group = None
         self._fused_ws = None
         self._fused_loss = None
+        self._fused_depth_loss = None
+        self._v_output_depth = None
 
     def set_view_cams(self, view_cams) -> None:
         """train.rs:172-174.  view_cams: sequence of ((x, y, z), focal_px) of the training views."""
@@ -287,7 +298,23 @@ class SplatTrainer:
         noise = self._host_rng.uniform(-s, s, 3).astype(np.float32)
         return tuple(float(x) for x in np.clip(base + noise, 0.0, 1.0))
 
+    def _depth_term(self, batch: SceneBatch) -> bool:
+        """Whether this step runs the depth term (DESIGN.md section 4.7): a positive weight and a map with valid pixels."""
+        return self.config.depth_loss_weight > 0.0 and batch.depth is not None and batch.depth_count > 0
+
+    def _depth_target(self, batch: SceneBatch) -> torch.Tensor:
+        img_h, img_w = batch.img_size()
+        t = batch.depth.to(self.ctx.device, non_blocking=True)
+        if t.dtype != torch.float32 or tuple(t.shape) != (img_h, img_w) or not t.is_contiguous():
+            raise ValueError(f"SceneBatch.depth must be a contiguous float32 [{img_h},{img_w}] tensor")
+        return t
+
+    def _depth_chain(self, batch: SceneBatch) -> float:
+        return float(np.float32(self.config.depth_loss_weight) / np.float32(batch.depth_count))   # w_d / |valid|, in f32
+
     def step(self, batch: SceneBatch, splats: Splats) -> TrainStepStats:
+        if self._depth_term(batch):
+            return self._step_depth(batch, splats)
         cfg = self.config
         self._ensure_state(splats)
         st = self._state
@@ -323,18 +350,59 @@ class SplatTrainer:
             self.grad_hook((v_t, v_sh, v_o, v_r, out.visible, out.max_radius))
 
         lr_mean = self._apply_updates(splats, v_t, v_sh, v_o, v_r, out.visible, out.max_radius, median_scale)
-        return TrainStepStats(num_visible_event=out, lr_mean=lr_mean, loss=loss)
+        depth_loss = torch.zeros((), dtype=torch.float32, device=dev) if batch.depth is not None else None
+        return TrainStepStats(num_visible_event=out, lr_mean=lr_mean, loss=loss, depth_loss=depth_loss)
+
+    def _step_depth(self, batch: SceneBatch, splats: Splats) -> TrainStepStats:
+        """step() with the depth term: depth render -> image loss -> depth loss (adds dL/dalpha to v_output[...,3]) ->
+        depth rasterize backward -> projection backward with v_z; the floor backward, the hook and the update as in step()."""
+        cfg = self.config
+        self._ensure_state(splats)
+        self.step_count += 1
+        img_h, img_w = batch.img_size()
+        dev = self.ctx.device
+        gt_packed = batch.img_packed.to(dev, non_blocking=True)
+        target = self._depth_target(batch)
+        background = self.sample_background()
+        median_scale = self.bounds.median_size()
+
+        r_transforms, r_raw_opac = splats.folded(self.ctx)
+        out = render_splats(self.ctx, batch.camera, (img_w, img_h), r_transforms, splats.sh_coeffs,
+                            r_raw_opac, mip=cfg.render_mip, background=background, rpass=PASS_BACKWARD, render_depth=True)
+        l1_w, ssim_w = (1.0 - cfg.ssim_weight, -cfg.ssim_weight) if self.ssim_enabled else (1.0, 0.0)
+        do_alpha_match = batch.has_alpha and not batch.masked_alpha and cfg.match_alpha_weight > 0.0
+        composite = background if (batch.has_alpha and any(b != 0.0 for b in background)) else None
+        lcfg = ImageLossConfig(l1_w, ssim_w, composite, batch.masked_alpha)
+        channels = 4 if do_alpha_match else 3
+        npx = float(img_h * img_w)
+        chain = [1.0 / (3.0 * npx)] * 3 + ([cfg.match_alpha_weight / npx] if do_alpha_match else [])
+        # a buffer of its own: the depth term writes channel 3, which the plain step's buffer keeps at zero
+        if self._v_output_depth is None or self._v_output_depth.shape != out.out_img.shape:
+            self._v_output_depth = torch.zeros_like(out.out_img)
+        elif channels == 3:
+            self._v_output_depth[..., 3].zero_()
+        v_output, loss = image_loss_fused(self.ctx, out.out_img, gt_packed, channels, lcfg, chain, self._v_output_depth)
+        v_depth, depth_loss = depth_loss_fused(self.ctx, out.out_img, out.depth, target, self._depth_chain(batch), v_output)
+        v_combined, v_z = rasterize_bwd_depth(out, v_output, v_depth)
+        v_t, v_sh, v_o, v_r = project_bwd(out, r_transforms, splats.sh_coeffs, r_raw_opac, v_combined, v_z=v_z)
+        if splats.min_scale is not None:
+            fold_min_scale_backward(self.ctx, splats.transforms, splats.raw_opacities, splats.min_scale, v_t, v_o)
+        if self.grad_hook is not None:
+            self.grad_hook((v_t, v_sh, v_o, v_r, out.visible, out.max_radius))
+
+        lr_mean = self._apply_updates(splats, v_t, v_sh, v_o, v_r, out.visible, out.max_radius, median_scale)
+        return TrainStepStats(num_visible_event=out, lr_mean=lr_mean, loss=loss + depth_loss, depth_loss=depth_loss)
 
 
     # ------------------------------------------------------------------------------------------------
     def step_fused(self, batch: SceneBatch, splats: Splats) -> TrainStepStats:
         """The same step through ONE ABI call (bg_train_step): every launch of the step is issued by the library on
-        the current stream, scratch comes from a workspace allocated once.  No min-scale floor, no gradient hook."""
+        the current stream, scratch comes from a workspace allocated once.  No min-scale floor, no gradient hook.
+        A batch that carries depth goes through bg_train_step_depth (the depth term of DESIGN.md section 4.7)."""
         if splats.min_scale is not None or self.grad_hook is not None:
             raise ValueError("step_fused handles the plain single-view step; use step() with a scale floor or a gradient hook")
         cfg = self.config
         self._ensure_state(splats)
-        st = self._state
         self.step_count += 1
         img_h, img_w = batch.img_size()
         dev = self.ctx.device
@@ -343,10 +411,34 @@ class SplatTrainer:
         background = self.sample_background()
         median_scale = self.bounds.median_size()
         n, k = splats.num_splats(), splats.sh_coeffs.shape[1]
-        need = int(lib.bg_train_step_workspace_bytes(n, k, img_w, img_h))
+        with_depth = batch.depth is not None
+        need = int((lib.bg_train_step_depth_workspace_bytes if with_depth else lib.bg_train_step_workspace_bytes)(n, k, img_w, img_h))
         if self._fused_ws is None or self._fused_ws.numel() < need:
             self._fused_ws = torch.empty(need, dtype=torch.uint8, device=dev)
             self._fused_loss = torch.zeros(1, dtype=torch.float32, device=dev)
+        a, lr_mean = self._fused_args(batch, splats, gt_packed, background, median_scale, self._fused_ws, need)
+        a.loss_out = self._fused_loss.data_ptr()
+        if not with_depth:
+            _lib.check(lib.bg_train_step(self.ctx.handle, _stream_ptr(dev), C.byref(a)), "bg_train_step")
+            return TrainStepStats(num_visible_event=None, lr_mean=lr_mean, loss=self._fused_loss[0])
+        # bg_train_step_depth runs bg_train_step itself when the term is off (weight 0 or no valid pixel)
+        if self._fused_depth_loss is None:
+            self._fused_depth_loss = torch.zeros(1, dtype=torch.float32, device=dev)
+        ds = _lib.BgDepthSupervision()
+        target = self._depth_target(batch) if self._depth_term(batch) else None
+        ds.target = target.data_ptr() if target is not None else None
+        ds.weight, ds.valid_count = float(cfg.depth_loss_weight), int(batch.depth_count)
+        ds.depth_loss_out = self._fused_depth_loss.data_ptr()
+        _lib.check(lib.bg_train_step_depth(self.ctx.handle, _stream_ptr(dev), C.byref(a), C.byref(ds)), "bg_train_step_depth")
+        self._fused_keepalive = target
+        return TrainStepStats(num_visible_event=None, lr_mean=lr_mean, loss=self._fused_loss[0],
+                              depth_loss=self._fused_depth_loss[0])
+
+    def _fused_args(self, batch: SceneBatch, splats: Splats, gt_packed, background, median_scale, ws, need):
+        """BgTrainStepArgs of step_fused for the current step_count (loss_out left unset)."""
+        cfg, st = self.config, self._state
+        img_h, img_w = batch.img_size()
+        n, k = splats.num_splats(), splats.sh_coeffs.shape[1]
         from .camera import build_uniforms
         a = _lib.BgTrainStepArgs()
         a.cam = _lib.camera_struct(build_uniforms(batch.camera, img_w, img_h))
@@ -369,10 +461,8 @@ class SplatTrainer:
         a.lr_coeffs_dc, a.lr_coeffs_sh_scale, a.lr_opac = cfg.lr_coeffs_dc, cfg.lr_coeffs_sh_scale, cfg.lr_opac
         a.noise_scale = float(np.float32(lr_mean) * np.float32(cfg.mean_noise_weight))
         a.median_scale, a.seed, a.step = float(median_scale), int(cfg.seed), self.step_count
-        a.workspace, a.workspace_bytes = self._fused_ws.data_ptr(), need
-        a.loss_out = self._fused_loss.data_ptr()
-        _lib.check(lib.bg_train_step(self.ctx.handle, _stream_ptr(dev), C.byref(a)), "bg_train_step")
-        return TrainStepStats(num_visible_event=None, lr_mean=lr_mean, loss=self._fused_loss[0])
+        a.workspace, a.workspace_bytes = ws.data_ptr(), need
+        return a, lr_mean
 
     # ------------------------------------------------------------------------------------------------
     def step_views(self, batches: Sequence[SceneBatch], splats: Splats, group=None, chunks: int = 0,
@@ -396,6 +486,8 @@ class SplatTrainer:
         local = len(batches)
         if local == 0 or local * world > 16:
             raise ValueError("step_views needs 1..16 views per step in total")
+        if cfg.depth_loss_weight > 0.0 and any(b.depth is not None for b in batches):
+            raise ValueError("step_views has no depth term: train views with depth through step() or step_fused()")
         if multi and (self._dp_comm is None or self._dp_group is not group):
             from .dp import DpComm
             self._dp_comm, self._dp_group = DpComm(self.ctx, group), group

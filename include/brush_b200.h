@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define BG_ABI_VERSION 6u
+#define BG_ABI_VERSION 7u
 
 /* f32 lanes per projected splat: a 64-byte row, four aligned 128-bit loads.  Lanes 0..8 are the reference
  * layout (kernels/helpers.rs:49-53: xy_x, xy_y, conic_x, conic_y, conic_z, color_a, color_r, color_g, color_b).
@@ -227,6 +227,37 @@ typedef struct {
 } BgTrainStepArgs;
 uint64_t bg_train_step_workspace_bytes(uint32_t n, uint32_t k, uint32_t w, uint32_t h);
 int32_t bg_train_step(BgContext *ctx, void *stream, BgTrainStepArgs *args);
+
+/* Depth supervision (DESIGN.md section 4.7; not a reference operator).  target: device [h,w] metric camera-space z of the
+ * view; a pixel is valid when its target is finite and > 0 (0 = no measurement).  With a = out_img[...,3], ed = D / a
+ * and a pixel active when it is valid and a >= 1/255, the term is
+ *   L_d = (weight / valid_count) * sum over active pixels of |ed - t|.
+ * valid_count is the number of valid pixels, counted by the host when the map was loaded (never read back here). */
+typedef struct {
+    const float *target;      /* device [h,w] f32; may be null when weight == 0 or valid_count == 0 */
+    float weight;             /* w_d >= 0, finite */
+    uint32_t valid_count;     /* |valid pixels| */
+    float *depth_loss_out;    /* device scalar: L_d (0 when the term is skipped) */
+} BgDepthSupervision;
+
+/* One pass of the depth term over a depth render (bg_render_forward_depth): with chain = weight / valid_count and
+ * s = sign(ed - t) (sign(0) = 0), writes v_depth = chain * s / a on active pixels and 0 elsewhere, ADDS -v_depth * ed to
+ * v_output[...,3] on active pixels only (that slot may already hold the image loss's alpha gradient), and writes per-block
+ * partial sums of |ed - t| (device float[bg_depth_loss_num_partials(h, w)]; L_d = chain * their sum).  IEEE division, no
+ * float atomics.  out_img and v_output: [h,w,4], 16-byte aligned.  chain must be finite and >= 0. */
+uint32_t bg_depth_loss_num_partials(uint32_t h, uint32_t w);
+int32_t bg_depth_loss_fused(BgContext *ctx, void *stream, const float *out_img /*[h,w,4]*/, const float *depth /*[h,w]*/,
+                            const float *target /*[h,w]*/, uint32_t h, uint32_t w, float chain /* w_d/|valid| */,
+                            float *v_output /*[h,w,4], channel 3 +=*/, float *v_depth /*[h,w]*/, float *partials);
+
+/* bg_train_step with the depth term: bg_render_forward_depth -> image loss -> bg_depth_loss_fused ->
+ * bg_rasterize_backward_depth -> bg_project_backward_depth -> the same update pass.  *args->loss_out = image loss + L_d;
+ * *depth->depth_loss_out = L_d.  Nothing is read back (capturable in a CUDA graph).  workspace:
+ * bg_train_step_depth_workspace_bytes(n, k, w, h) bytes (else BG_ERR_CAPACITY).  weight == 0 or valid_count == 0 runs
+ * bg_train_step itself (bit-identical results) and writes 0 to depth_loss_out.  A negative or non-finite weight is
+ * BG_ERR_INVALID; a null args, depth or depth_loss_out (or a null target when the term runs) is BG_ERR_NULL. */
+uint64_t bg_train_step_depth_workspace_bytes(uint32_t n, uint32_t k, uint32_t w, uint32_t h);
+int32_t bg_train_step_depth(BgContext *ctx, void *stream, BgTrainStepArgs *args, const BgDepthSupervision *depth);
 
 /* The parameter update of one step as ONE pass over the Gaussians (update.cu): AdamScaled::step on the three parameter
  * tensors (brush-train/src/adam_scaled.rs:75-165, train.rs:328-381), RefineRecord::gather_stats (stats.rs:40-50) and the

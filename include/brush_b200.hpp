@@ -439,6 +439,8 @@ struct TrainConfig {                         // brush-train/src/config.rs:5-132 
     float growth_grad_threshold = 0.0025f, growth_select_fraction = 0.25f;
     uint32_t growth_stop_iter = 15000;
     float split_at_screen_size = 0.5f;
+    // depth supervision (DESIGN.md section 4.7): weight of the L1 term on the expected depth; 0 = the plain step
+    float depth_loss_weight = 0.0f;
 };
 
 // brush-render/src/bounding_box.rs:5-31
@@ -543,8 +545,39 @@ class SplatTrainer {
     // gt_packed: device [h,w] rgba8 (view_to_packed_data, scene.rs:97-136).  Returns the device scalar holding the loss.
     const float *step(Context &ctx, cudaStream_t stream, const Camera &camera, const uint32_t *gt_packed, uint32_t w, uint32_t h,
                       float *transforms, float *sh_coeffs, float *raw_opacities, bool has_alpha = false, bool masked_alpha = false) {
+        BgTrainStepArgs a = step_args(camera, gt_packed, w, h, transforms, sh_coeffs, raw_opacities, has_alpha, masked_alpha,
+                                      bg_train_step_workspace_bytes(n_, k_, w, h));
+        check(bg_train_step(ctx.handle(), stream, &a), "SplatTrainer::step");
+        last_state_ = a.state_out;
+        return loss_.data();
+    }
+    // The step with depth supervision (bg_train_step_depth, DESIGN.md section 4.7): depth_target is the view's device [h,w]
+    // metric camera-space z (0 = no measurement), depth_valid_count its number of valid pixels.  With
+    // cfg.depth_loss_weight == 0 or no valid pixel this is the plain step.  Returns the device scalars
+    // (loss = image loss + depth loss, depth loss).
+    struct StepLosses {
+        const float *loss;
+        const float *depth_loss;
+    };
+    StepLosses step(Context &ctx, cudaStream_t stream, const Camera &camera, const uint32_t *gt_packed, const float *depth_target,
+                    uint32_t depth_valid_count, uint32_t w, uint32_t h, float *transforms, float *sh_coeffs, float *raw_opacities,
+                    bool has_alpha = false, bool masked_alpha = false) {
+        BgTrainStepArgs a = step_args(camera, gt_packed, w, h, transforms, sh_coeffs, raw_opacities, has_alpha, masked_alpha,
+                                      bg_train_step_depth_workspace_bytes(n_, k_, w, h));
+        BgDepthSupervision d;
+        d.target = depth_target;
+        d.weight = cfg_.depth_loss_weight;
+        d.valid_count = depth_valid_count;
+        d.depth_loss_out = depth_loss_.data();
+        check(bg_train_step_depth(ctx.handle(), stream, &a, &d), "SplatTrainer::step (depth)");
+        last_state_ = a.state_out;
+        return {loss_.data(), depth_loss_.data()};
+    }
+
+   private:
+    BgTrainStepArgs step_args(const Camera &camera, const uint32_t *gt_packed, uint32_t w, uint32_t h, float *transforms,
+                              float *sh_coeffs, float *raw_opacities, bool has_alpha, bool masked_alpha, uint64_t need) {
         step_ += 1;
-        const uint64_t need = bg_train_step_workspace_bytes(n_, k_, w, h);
         if (ws_.size() < need) ws_ = DeviceBuffer<unsigned char>(need);
         BgTrainStepArgs a;
         std::memset(&a, 0, sizeof(a));
@@ -574,10 +607,10 @@ class SplatTrainer {
         a.step = step_;
         a.workspace = ws_.data(); a.workspace_bytes = need;
         a.loss_out = loss_.data();
-        check(bg_train_step(ctx.handle(), stream, &a), "SplatTrainer::step");
-        last_state_ = a.state_out;
-        return loss_.data();
+        return a;
     }
+
+   public:
     // One optimizer step over several views (SURVEY.md 8e, BASELINE config [4]) through bg_train_step_views: the loss is the
     // mean of the per-view losses.  `comm` == nullptr: all views on this device.  With a communicator every rank passes ITS
     // views (the same count on every rank; global view index = rank * local + i) and all ranks end with bit-identical
@@ -701,6 +734,7 @@ class SplatTrainer {
     double decay_ = 1.0;
     int step_ = 0;
     DeviceBuffer<float> m_t_, v_t_, m_sh_, v_sh_, m_o_, v_o_, refine_norm_, vis_weight_, max_screen_, loss_;
+    DeviceBuffer<float> depth_loss_{1, true};
     DeviceBuffer<unsigned char> ws_, views_ws_;
     BgRenderState last_state_{};
     BoundingBox bounds_;

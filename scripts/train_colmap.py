@@ -11,6 +11,12 @@
   3. reported: iterations / s (whole run, wall clock, refine and data loading included), PSNR / SSIM on the held-out
      views, the splat count after every refine.
 
+With --depth-loss-weight W > 0 the set also gets depths/view_XXXX.png: 16-bit millimetres of the hidden scene's expected
+depth D / alpha on covered pixels (alpha >= 0.5), 0 elsewhere; the run trains with the depth term (DESIGN.md section
+4.7) and the evaluation adds depth_abs_rel / depth_rmse / depth_coverage.  W = 0 (the default) writes and runs exactly
+what it did before.  --write-depths writes the depth maps at W = 0 too (the plain step; evaluation reports the depth
+figures).
+
   python scripts/train_colmap.py --iters 3000 --views 200 --init-points 500000 --max-splats 2000000
 """
 from __future__ import annotations
@@ -60,8 +66,9 @@ def colmap_pose(cam):
     return q, tuple(float(v) for v in t)
 
 
-def make_dataset(root: str, ctx, views: int, w: int, h: int, hidden_n: int, init_points: int, seed: int = 0xB2000002):
-    """Writes the COLMAP-format set under `root`; returns (hidden scene arrays, cameras)."""
+def make_dataset(root: str, ctx, views: int, w: int, h: int, hidden_n: int, init_points: int, seed: int = 0xB2000002,
+                 depth: bool = False):
+    """Writes the COLMAP-format set under `root` (with depth: also depths/*.png); returns (hidden scene arrays, cameras)."""
     import torch
     from PIL import Image
     import brush_b200.render as R
@@ -88,6 +95,13 @@ def make_dataset(root: str, ctx, views: int, w: int, h: int, hidden_n: int, init
         rgba = out.out_img.cpu().numpy().view(np.uint8).reshape(h, w, 4)
         rgb = np.ascontiguousarray(rgba[..., :3])
         jobs.append(pool.submit(lambda a, p: Image.fromarray(a).save(p, compress_level=1), rgb, os.path.join(root, "images", name)))
+        if depth:
+            dout = R.render_splats(ctx, cam, (w, h), ttr, tsh, top, rpass=R.PASS_BACKWARD, render_depth=True)
+            a = dout.out_img[..., 3]
+            ed = torch.where(a >= 0.5, dout.depth / a.clamp_min(1e-30), torch.zeros_like(a))
+            mm = (ed * 1000.0).round().clamp(0, 65535).to(torch.int32).cpu().numpy().astype(np.uint16)
+            os.makedirs(os.path.join(root, "depths"), exist_ok=True)
+            jobs.append(pool.submit(lambda a, p: Image.fromarray(a).save(p, compress_level=1), mm, os.path.join(root, "depths", name)))
         q, t = colmap_pose(cam)
         lines.append(f"{i + 1} {q[0]!r} {q[1]!r} {q[2]!r} {q[3]!r} {t[0]!r} {t[1]!r} {t[2]!r} 1 {name}\n\n")
     with open(os.path.join(sparse, "images.txt"), "w") as f:
@@ -109,7 +123,7 @@ def make_dataset(root: str, ctx, views: int, w: int, h: int, hidden_n: int, init
 
 def run(device: int = 0, iters: int = 3000, views: int = 200, width: int = 1920, height: int = 1080, hidden_n: int = 1_000_000,
         init_points: int = 500_000, max_splats: int = 2_000_000, refine_every: int = None, root: str = None, quiet: bool = False,
-        keep: bool = False) -> dict:
+        keep: bool = False, depth_loss_weight: float = 0.0, write_depths: bool = False) -> dict:
     import torch
     import brush_b200.render as R
     import brush_b200.train as T
@@ -122,7 +136,7 @@ def run(device: int = 0, iters: int = 3000, views: int = 200, width: int = 1920,
     root = root or tempfile.mkdtemp(prefix="bg_colmap_")
     ctx = R.RenderContext(max_splats, width, height, 0, device=device)
     t0 = time.time()
-    make_dataset(root, ctx, views, width, height, hidden_n, init_points)
+    make_dataset(root, ctx, views, width, height, hidden_n, init_points, depth=depth_loss_weight > 0 or write_depths)
     t_data = time.time() - t0
     say(f"dataset: {views} views {width}x{height} in {t_data:.1f} s -> {root}")
     t0 = time.time()
@@ -136,7 +150,7 @@ def run(device: int = 0, iters: int = 3000, views: int = 200, width: int = 1920,
     if refine_every is None:
         refine_every = 200 if iters >= 2000 else max(50, iters // 6)
     cfg = T.TrainConfig(total_train_iters=iters, max_splats=max_splats, refine_every=refine_every,
-                        growth_stop_iter=max(int(iters * 0.8), 1), seed=1)
+                        growth_stop_iter=max(int(iters * 0.8), 1), seed=1, depth_loss_weight=depth_loss_weight)
     counts, step_ms = [], []
     marks = {"t": None, "done": 0}
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -164,6 +178,8 @@ def run(device: int = 0, iters: int = 3000, views: int = 200, width: int = 1920,
            "final_splats": splats.num_splats(), "splats_after_refine": counts,
            "step_windows": [{"steps": s, "ms_per_step": ms / s, "splats": n} for s, ms, n in step_ms],
            "eval": evals[-1] if evals else None}
+    if depth_loss_weight > 0:
+        res["depth_loss_weight"] = depth_loss_weight
     if step_ms:
         res["iters_per_s_steps_only"] = sum(s for s, _, _ in step_ms) / (sum(ms for _, ms, _ in step_ms) * 1e-3)
     say(json.dumps(res))
@@ -185,7 +201,10 @@ if __name__ == "__main__":
     ap.add_argument("--refine-every", type=int, default=None)
     ap.add_argument("--root", default=None)
     ap.add_argument("--keep", action="store_true")
+    ap.add_argument("--depth-loss-weight", type=float, default=0.0)
+    ap.add_argument("--write-depths", action="store_true")
     a = ap.parse_args()
     r = run(iters=a.iters, views=a.views, width=a.width, height=a.height, hidden_n=a.hidden, init_points=a.init_points,
-            max_splats=a.max_splats, refine_every=a.refine_every, root=a.root, keep=a.keep)
+            max_splats=a.max_splats, refine_every=a.refine_every, root=a.root, keep=a.keep, depth_loss_weight=a.depth_loss_weight,
+            write_depths=a.write_depths)
     print(json.dumps(r))
