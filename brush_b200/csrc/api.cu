@@ -18,17 +18,16 @@
 
 namespace bg {
 // project.cu
-cudaError_t launch_project_cull(cudaStream_t, int, bool, const float *, const float *, uint32_t, const BgCamera &,
-                                uint32_t, uint32_t, uint32_t, uint32_t, uint32_t *, uint32_t *, uint32_t *, float *,
-                                uint32_t *, unsigned long long *, uint32_t *, unsigned long long *, const uint32_t *,
-                                uint32_t);
+cudaError_t launch_project_cull(cudaStream_t, int, bool, int, const float *, const float *, const float *, uint32_t,
+                                const BgCamera &, uint32_t, uint32_t, uint32_t, uint32_t, uint32_t *, uint32_t *,
+                                uint32_t *, float *, uint32_t *, float *, uint32_t *, unsigned long long *,
+                                const uint32_t *, uint32_t);
 cudaError_t launch_gather_scan(cudaStream_t, int, const uint32_t *, const uint32_t *, uint32_t, const uint32_t *,
                                uint32_t *, uint32_t *, uint32_t, uint32_t *, uint32_t *, unsigned long long *,
                                const uint32_t *, uint32_t);
-cudaError_t launch_project_visible_emit(cudaStream_t, int, bool, int, const float *, const float *, const float *,
-                                        const uint32_t *, const uint32_t *, const BgCamera &, uint32_t, uint32_t,
-                                        float *, uint32_t *, uint32_t *, uint32_t, uint32_t *, const unsigned long long *,
-                                        uint32_t *, uint32_t);
+cudaError_t launch_project_visible_emit(cudaStream_t, int, const float *, const uint32_t *, const uint32_t *, uint32_t,
+                                        uint32_t, float *, uint32_t *, uint32_t *, uint32_t, uint32_t *, uint32_t *,
+                                        uint32_t);
 cudaError_t launch_tile_offsets(cudaStream_t, int, const uint32_t *, const uint32_t *, uint32_t, uint32_t *);
 // sort.cu
 cudaError_t launch_radix_hist(cudaStream_t, int, const uint32_t *, uint32_t, const uint32_t *, uint32_t, uint32_t,
@@ -113,7 +112,7 @@ struct BgContext {
     uint32_t *depth_key[2] = {nullptr, nullptr};
     uint32_t *depth_val[2] = {nullptr, nullptr};
     uint32_t *counts = nullptr, *cum = nullptr, *cgid_from_gid = nullptr;
-    unsigned long long *hit_masks = nullptr;  // per-Gaussian tile hit bits from the counting pass
+    float *row_by_gid = nullptr;  // [N,16] projected rows by global id + tile hit bits (project_cull -> emit)
     float *projected = nullptr;
     uint32_t *isect_key[2] = {nullptr, nullptr};
     uint32_t *isect_val[2] = {nullptr, nullptr};
@@ -150,7 +149,7 @@ extern "C" int32_t bg_ctx_destroy(BgContext *c) {
     if (!c) return BG_ERR_NULL;
     cudaSetDevice(c->device);
     void *ptrs[] = {c->ctl, c->depth_key[0], c->depth_key[1], c->depth_val[0], c->depth_val[1], c->counts, c->cum,
-                    c->cgid_from_gid, c->hit_masks, c->projected, c->isect_key[0], c->isect_key[1], c->isect_val[0], c->isect_val[1],
+                    c->cgid_from_gid, c->row_by_gid, c->projected, c->isect_key[0], c->isect_key[1], c->isect_val[0], c->isect_val[1],
                     c->tile_offsets, c->lb_scan, c->lb_sort, c->epoch_dev, c->live_masks, c->warp_batches, c->blend_stats};
     for (void *p : ptrs)
         if (p) cudaFree(p);
@@ -193,7 +192,7 @@ extern "C" int32_t bg_ctx_create(int32_t device, uint32_t max_splats, uint32_t m
     ok = ok && arena_alloc(c, &c->counts, n) == cudaSuccess;
     ok = ok && arena_alloc(c, &c->cum, n) == cudaSuccess;
     ok = ok && arena_alloc(c, &c->cgid_from_gid, n) == cudaSuccess;
-    ok = ok && arena_alloc(c, &c->hit_masks, n) == cudaSuccess;
+    ok = ok && arena_alloc(c, &c->row_by_gid, n * BG_PROJECTED_STRIDE) == cudaSuccess;
     ok = ok && arena_alloc(c, &c->projected, n * BG_PROJECTED_STRIDE) == cudaSuccess;
     ok = ok && arena_alloc(c, &c->tile_offsets, (uint64_t)c->max_tiles * 2) == cudaSuccess;
     ok = ok && arena_alloc(c, &c->live_masks, (I / 32 + c->max_tiles + 2) * 4) == cudaSuccess;
@@ -278,12 +277,12 @@ static int32_t render_forward(BgContext *c, void *stream, const BgCamera *cam, u
     if (bwd_info && n > 0) BG_CUDA(cudaMemsetAsync(visible, 0, (size_t)n * sizeof(float), s));
 
     const int pgrid = c->sm_count * 5;   // project_cull: 256-thread CTAs, 48 regs
-    const int vgrid = c->sm_count * 6;   // project_visible_emit: 128-thread CTAs (8 CTAs/SM would force 64 regs and spill)
+    const int vgrid = c->sm_count * 8;   // project_visible_emit: 128-thread CTAs, __launch_bounds__(128, 8) (project.cu)
     uint32_t *counters = c->ctl + CTL_COUNTERS;
-    // K1: cull + compaction in index order
-    BG_CUDA(launch_project_cull(s, pgrid, mip != 0, transforms, raw_opac, n, *cam, w, h, tiles_x, tiles_y,
-                                c->depth_key[0], c->depth_val[0], c->counts, max_radius, c->cgid_from_gid, c->hit_masks, c->ctl,
-                                c->lb_scan, c->epoch_dev, EP_PROJECT));
+    // K1: cull + compaction in index order; finished projected rows (colour included) staged by global id
+    BG_CUDA(launch_project_cull(s, pgrid, mip != 0, deg, transforms, sh, raw_opac, n, *cam, w, h, tiles_x, tiles_y,
+                                c->depth_key[0], c->depth_val[0], c->counts, max_radius, c->cgid_from_gid, c->row_by_gid,
+                                c->ctl, c->lb_scan, c->epoch_dev, EP_PROJECT));
     // depth sort: 32-bit keys, 4 passes, (0)->(1)->(0)->(1)->(0)
     int dout = 0;
     {
@@ -302,9 +301,9 @@ static int32_t render_forward(BgContext *c, void *stream, const BgCamera *cam, u
     while (bits < 32 && (num_tiles >> bits) != 0) bits++;
     // K2+K3 (also counts the tile-key digits for the sort when they fit two passes)
     if (n > 0)
-        BG_CUDA(launch_project_visible_emit(s, vgrid, mip != 0, deg, transforms, sh, raw_opac, gid_sorted, c->cum, *cam,
-                                            tiles_x, tiles_y, c->projected, c->isect_key[0], c->isect_val[0],
-                                            c->max_isect, c->cgid_from_gid, c->hit_masks, c->ctl, bits));
+        BG_CUDA(launch_project_visible_emit(s, vgrid, c->row_by_gid, gid_sorted, c->cum, tiles_x, tiles_y, c->projected,
+                                            c->isect_key[0], c->isect_val[0], c->max_isect, c->cgid_from_gid, c->ctl,
+                                            bits));
     int iout = 0;
     {
         const uint32_t passes = (bits + 7) / 8;

@@ -14,7 +14,8 @@
 //   * compaction of visible Gaussians is a single-pass decoupled look-back in index order --
 //     deterministic, unlike the reference's atomic slot (project_forward.rs:122-124);
 //   * the [n,10] AoS rows of a tile are staged with one TMA bulk copy (cp.async.bulk + mbarrier),
-//     double buffered; gathered rows (SH, transforms by sorted id) are read as whole 32-byte sectors.
+//     double buffered; the SH rows are read in index order there too, and the depth-ordered pass gathers one
+//     64-byte staged row per splat (two whole 32-byte sectors).
 #include "bg_project.cuh"
 
 namespace bg {
@@ -29,6 +30,7 @@ struct CullResult {
     unsigned long long mask;  // hit bits of the bbox tiles, row major, valid when the bbox has <= 64 tiles
     // screen-space footprint, consumed by the warp-cooperative tile count
     float mx, my, c00, c01, c11, pt;
+    float opac;               // compensated opacity, lane 5 of the projected row
     uint32_t min_x, min_y, bbw, ntiles;
 };
 
@@ -38,7 +40,7 @@ __device__ __forceinline__ CullResult cull_one(const float *t, float raw_opac, c
                                                uint32_t img_h, uint32_t tiles_x, uint32_t tiles_y) {
     CullResult r;
     r.visible = false; r.depth = 0.0f; r.tiles = 0; r.radius = 0.0f; r.mask = 0ull;
-    r.mx = r.my = r.c00 = r.c01 = r.c11 = r.pt = 0.0f;
+    r.mx = r.my = r.c00 = r.c01 = r.c11 = r.pt = r.opac = 0.0f;
     r.min_x = r.min_y = r.bbw = r.ntiles = 0;
     V3 mean_c = world_to_cam(mk3(t[0], t[1], t[2]), u);
     if (!(is_finite(mean_c) && mean_c.z <= 1.0e10f)) return r;
@@ -70,7 +72,7 @@ __device__ __forceinline__ CullResult cull_one(const float *t, float raw_opac, c
     r.visible = true;
     r.depth = mean_c.z;
     r.radius = fmaxf(ex / wf, ey / hf);
-    r.mx = mx; r.my = my; r.c00 = conic.c00; r.c01 = conic.c01; r.c11 = conic.c11; r.pt = pt;
+    r.mx = mx; r.my = my; r.c00 = conic.c00; r.c01 = conic.c01; r.c11 = conic.c11; r.pt = pt; r.opac = opac;
     r.min_x = bb.min_x; r.min_y = bb.min_y; r.bbw = bb.max_x - bb.min_x;
     r.ntiles = (bb.max_y - bb.min_y) * r.bbw;
     return r;
@@ -131,14 +133,47 @@ __device__ __forceinline__ void warp_count_tiles(CullResult &r) {
     r.mask = mask;
 }
 
+// Colour of one splat (+0.5, non-finite -> 0, clamped), its SH row read in 128-bit pieces where the row is 16-byte
+// aligned (K = 1, 9 rows are read float by float).
+template <int DEG>
+__device__ __forceinline__ V3 splat_color(const float *__restrict__ sh, uint32_t gid, V3 vdir) {
+    constexpr int KF = (DEG + 1) * (DEG + 1) * 3;        // floats per SH row
+    float coef[KF];
+    if ((KF % 4) == 0) {                                 // rows of 48 B / 192 B are 16-byte aligned
+        const float4 *row4 = reinterpret_cast<const float4 *>(sh + (size_t)gid * KF);
+#pragma unroll
+        for (int i = 0; i < KF / 4; i++) {
+            float4 q = __ldg(row4 + i);
+            coef[4 * i] = q.x; coef[4 * i + 1] = q.y; coef[4 * i + 2] = q.z; coef[4 * i + 3] = q.w;
+        }
+    } else {
+        const float *row = sh + (size_t)gid * KF;
+#pragma unroll
+        for (int i = 0; i < KF; i++) coef[i] = __ldg(row + i);
+    }
+    V3 raw = sh_to_color<DEG>([&](int i) { return coef[i]; }, vdir);
+    float cr = raw.x + 0.5f, cg = raw.y + 0.5f, cb = raw.z + 0.5f;
+    cr = clampf(is_finite(cr) ? cr : 0.0f, -100.0f, 100.0f);
+    cg = clampf(is_finite(cg) ? cg : 0.0f, -100.0f, 100.0f);
+    cb = clampf(is_finite(cb) ? cb : 0.0f, -100.0f, 100.0f);
+    return mk3(cr, cg, cb);
+}
+
 // K1.  One thread per Gaussian, 256 Gaussians per tile, persistent CTAs.
-template <bool MIP, bool DIST>
-__global__ void __launch_bounds__(PROJ_THREADS)
-project_cull_kernel(const float *__restrict__ transforms, const float *__restrict__ raw_opac, uint32_t n,
+// Each visible splat's finished projected row (lanes 0-12, the layout of `projected`, DESIGN §3) is written here, in
+// index order, to the gid-indexed staging rows `row_by_gid`, with the tile hit mask in lanes 13-14: the SH row is then a
+// streamed read, and the depth-ordered emit pass gathers one 64-byte row per splat instead of the parameter rows.
+// Pinhole: 5 CTAs per SM (48 registers, no spill) as before the colour moved here -- uncapped, the SH row takes the
+// kernel to 52-64 registers and 4 CTAs.  Distorted models are left to the compiler (64-80 registers, no spill): capped
+// at 64 their DEG >= 3 instantiations spill.
+template <bool MIP, int DEG, bool DIST>
+__global__ void __launch_bounds__(PROJ_THREADS, DIST ? 0 : 5)
+project_cull_kernel(const float *__restrict__ transforms, const float *__restrict__ sh,
+                    const float *__restrict__ raw_opac, uint32_t n,
                     BgCamera u, uint32_t img_w, uint32_t img_h, uint32_t tiles_x, uint32_t tiles_y,
                     uint32_t *__restrict__ depth_keys, uint32_t *__restrict__ gids,
                     uint32_t *__restrict__ counts_by_gid, float *__restrict__ max_radius,
-                    uint32_t *__restrict__ cgid_from_gid, unsigned long long *__restrict__ hit_masks,
+                    uint32_t *__restrict__ cgid_from_gid, float *__restrict__ row_by_gid,
                     uint32_t *__restrict__ ctl,
                     unsigned long long *__restrict__ lb_state, const uint32_t *__restrict__ epoch_base, uint32_t epoch_off) {
     // look-back epoch = (per-context call counter kept ON THE DEVICE) * 32 + launch index inside the call: nothing
@@ -188,8 +223,9 @@ project_cull_kernel(const float *__restrict__ transforms, const float *__restric
         const uint32_t gid = base + threadIdx.x;
         CullResult r;
         r.visible = false; r.depth = 0.0f; r.tiles = 0; r.radius = 0.0f; r.mask = 0ull;
-        r.mx = r.my = r.c00 = r.c01 = r.c11 = r.pt = 0.0f;
+        r.mx = r.my = r.c00 = r.c01 = r.c11 = r.pt = r.opac = 0.0f;
         r.min_x = r.min_y = r.bbw = r.ntiles = 0;
+        float4 *row = reinterpret_cast<float4 *>(row_by_gid + (size_t)gid * BG_PROJECTED_STRIDE);
         if (threadIdx.x < rows) {
             float t[10];
 #pragma unroll
@@ -197,6 +233,15 @@ project_cull_kernel(const float *__restrict__ transforms, const float *__restric
             r = cull_one<MIP, DIST>(t, __ldg(raw_opac + gid), u, img_w, img_h, tiles_x, tiles_y);
             max_radius[gid] = r.radius;  // zero for culled splats (render_aux.rs:76-78)
             cgid_from_gid[gid] = 0xFFFFFFFFu;  // overwritten for visible splats by project_visible_emit
+            // colour and row before the tile walk, so the SH coefficients are dead while it runs
+            if (r.visible) {
+                const V3 vdir = normalize(sub(mk3(t[0], t[1], t[2]), mk3(u.cam_pos[0], u.cam_pos[1], u.cam_pos[2])));
+                const V3 col = splat_color<DEG>(sh, gid, vdir);
+                const float L2E = 1.4426950408889634f;
+                row[0] = make_float4(r.mx, r.my, r.c00, r.c01);
+                row[1] = make_float4(r.c11, r.opac, col.x, col.y);
+                row[2] = make_float4(col.z, (0.5f * L2E) * r.c11, (0.5f * L2E) * r.c00, L2E * r.c01);
+            }
         }
         // The visible count is known before the (expensive) tile walk: publish the tile aggregate
         // first, count tiles, and only then look back -- by then the predecessors have published,
@@ -223,7 +268,7 @@ project_cull_kernel(const float *__restrict__ transforms, const float *__restric
             for (int p = 0; p < 4; p++) atomicAdd(&s_dhist[p * 256 + ((dk >> (8 * p)) & 255u)], 1u);
             gids[slot] = gid;
             counts_by_gid[gid] = r.tiles;
-            hit_masks[gid] = r.mask;
+            row[3] = make_float4(r.pt, __uint_as_float((uint32_t)r.mask), __uint_as_float((uint32_t)(r.mask >> 32)), 0.0f);
         }
         tile = s_tile_next;
         buf ^= 1u;
@@ -306,30 +351,31 @@ gather_scan_kernel(const uint32_t *__restrict__ in, const uint32_t *__restrict__
 
 // K2 + K3.  One thread per visible Gaussian in depth order (compact gid = position in the
 // depth-sorted list); WARPS are the unit of work (a ticket = 32 consecutive compact ids), so the loop has no
-// block barrier.  Every lane gathers its own parameter rows (the gather is by sorted global id, so
-// neighbouring lanes touch unrelated rows anyway): the 192-byte SH row as twelve independent 128-bit loads.
-// The kernel is bound by gather latency (long-scoreboard stalls on the first use of the rows), hence:
+// block barrier.  Every lane gathers the 64-byte staged row `project_cull_kernel` wrote for its splat (the gather is
+// by sorted global id, so neighbouring lanes touch unrelated rows anyway) as four 128-bit loads, copies lanes 0-12 to
+// `projected[cgid]` and emits the splat's intersections; the bbox is recomputed from the row (the same inputs and
+// functions as the cull), the small-bbox hits come from the mask in lanes 13-14.
+// The kernel is bound by gather latency (long-scoreboard stalls on the first use of the row), hence:
 //   * the NEXT ticket and its global ids are fetched at the top of an iteration, and the rows they point at are
 //     pulled into L2 with cp.async.bulk.prefetch.L2 while the current splats are processed;
 //   * the (tile id, compact gid) pairs of a warp -- one contiguous output range -- are gathered in shared memory
 //     and written with coalesced stores; bboxes larger than the 64-bit hit mask are tested by the whole warp.
+// Residency: the 22.5 KB of emission staging per 128-thread CTA allow 9 CTAs per SM; __launch_bounds__(128, 8) caps the
+// kernel at 64 registers (it uses 63, no spill), and the grid is 8 CTAs per SM (api.cu).  Measured on an H100 (400 W
+// limit), 1M splats at 1080p: 169 us, against 354 us for the former gather-and-recompute kernel at 6 CTAs per SM
+// (DESIGN §6.8).
 constexpr int VIS_THREADS = 128;
 
 __device__ __forceinline__ void prefetch_l2_bulk(const void *p, uint32_t bytes) {  // p 16-byte aligned, bytes % 16 == 0
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
 }
 
-template <bool MIP, int DEG, bool DIST>
-__global__ void __launch_bounds__(VIS_THREADS, 6)
-project_visible_emit_kernel(const float *__restrict__ transforms, const float *__restrict__ sh,
-                            const float *__restrict__ raw_opac, const uint32_t *__restrict__ gid_sorted,
-                            const uint32_t *__restrict__ cum, BgCamera u, uint32_t tiles_x, uint32_t tiles_y,
+__global__ void __launch_bounds__(VIS_THREADS, 8)
+project_visible_emit_kernel(const float *__restrict__ row_by_gid, const uint32_t *__restrict__ gid_sorted,
+                            const uint32_t *__restrict__ cum, uint32_t tiles_x, uint32_t tiles_y,
                             float *__restrict__ projected, uint32_t *__restrict__ tile_keys,
                             uint32_t *__restrict__ isect_vals, uint32_t isect_capacity,
-                            uint32_t *__restrict__ cgid_from_gid, const unsigned long long *__restrict__ hit_masks,
-                            uint32_t *__restrict__ ctl, uint32_t tile_bits) {
-    constexpr int KF = (DEG + 1) * (DEG + 1) * 3;        // floats per SH row
-    constexpr bool VEC4 = (KF % 4) == 0;                 // rows of 48 B / 192 B are 16-byte aligned
+                            uint32_t *__restrict__ cgid_from_gid, uint32_t *__restrict__ ctl, uint32_t tile_bits) {
     constexpr uint32_t EMIT_BUF = 1024;                  // staged (tile id, owner) pairs per warp
     __shared__ uint32_t s_emit_keys[(VIS_THREADS / 32) * EMIT_BUF];
     __shared__ uint8_t s_emit_own[(VIS_THREADS / 32) * EMIT_BUF];
@@ -374,64 +420,25 @@ project_visible_emit_kernel(const float *__restrict__ transforms, const float *_
         float e_mx = 0.f, e_my = 0.f, e_pt = 0.f;
         S2 e_conic; e_conic.c00 = e_conic.c01 = e_conic.c11 = 0.f;
         if (active) {
-            float coef[KF];
-            if (VEC4) {
-                const float4 *row4 = reinterpret_cast<const float4 *>(sh + (size_t)gid * KF);
-#pragma unroll
-                for (int i = 0; i < KF / 4; i++) {
-                    float4 q = __ldg(row4 + i);
-                    coef[4 * i] = q.x; coef[4 * i + 1] = q.y; coef[4 * i + 2] = q.z; coef[4 * i + 3] = q.w;
-                }
-            } else {
-                const float *row = sh + (size_t)gid * KF;
-#pragma unroll
-                for (int i = 0; i < KF; i++) coef[i] = __ldg(row + i);
-            }
-            const float2 *t2 = reinterpret_cast<const float2 *>(transforms + (size_t)gid * 10);
-            float2 a0 = __ldg(t2), a1 = __ldg(t2 + 1), a2 = __ldg(t2 + 2), a3 = __ldg(t2 + 3), a4 = __ldg(t2 + 4);
-            const float ro = __ldg(raw_opac + gid);
-            hitm = __ldg(hit_masks + gid);
+            const float4 *src = reinterpret_cast<const float4 *>(row_by_gid + (size_t)gid * BG_PROJECTED_STRIDE);
+            const float4 q0 = __ldg(src), q1 = __ldg(src + 1), q2 = __ldg(src + 2), q3 = __ldg(src + 3);
             base = (cgid == 0) ? 0u : __ldg(cum + cgid - 1);
             budget = __ldg(cum + cgid) - base;
-            V3 mean = mk3(a0.x, a0.y, a1.x);
-            Q4 qu; qu.w = a1.y; qu.x = a2.x; qu.y = a2.y; qu.z = a3.x;
-            V3 scl = mk3(det_expf(a3.y), det_expf(a4.x), det_expf(a4.y));
-            Q4 quat = normalize(qu);
-            V3 mean_c = world_to_cam(mean, u);
-            S2 raw_cov = calc_cov2d<DIST>(scl, quat, mean_c, u);
-            float comp;
-            S2 cov = compensate_cov2d<MIP>(raw_cov, comp);
-            float opac = det_sigmoid(ro) * comp;
-            S2 conic = inverse(cov);
-            float mx, my;
-            project_mean<DIST>(mean_c, u, mx, my);
-            V3 vdir = normalize(sub(mean, mk3(u.cam_pos[0], u.cam_pos[1], u.cam_pos[2])));
-            V3 raw = sh_to_color<DEG>([&](int i) { return coef[i]; }, vdir);
-            float cr = raw.x + 0.5f, cg = raw.y + 0.5f, cb = raw.z + 0.5f;
-            cr = clampf(is_finite(cr) ? cr : 0.0f, -100.0f, 100.0f);
-            cg = clampf(is_finite(cg) ? cg : 0.0f, -100.0f, 100.0f);
-            cb = clampf(is_finite(cb) ? cb : 0.0f, -100.0f, 100.0f);
-            float pt = det_logf(opac * 255.0f);
             float4 *dst = reinterpret_cast<float4 *>(projected + (size_t)cgid * BG_PROJECTED_STRIDE);
-            const float L2E = 1.4426950408889634f;
-            dst[0] = make_float4(mx, my, conic.c00, conic.c01);
-            dst[1] = make_float4(conic.c11, opac, cr, cg);
-            dst[2] = make_float4(cb, (0.5f * L2E) * conic.c11, (0.5f * L2E) * conic.c00, L2E * conic.c01);
-            dst[3] = make_float4(pt, 0.0f, 0.0f, 0.0f);
+            dst[0] = q0;
+            dst[1] = q1;
+            dst[2] = q2;
+            dst[3] = make_float4(q3.x, 0.0f, 0.0f, 0.0f);
             cgid_from_gid[gid] = cgid;
+            hitm = (unsigned long long)__float_as_uint(q3.y) | ((unsigned long long)__float_as_uint(q3.z) << 32);
             // ---- (tile id, compact gid) pairs (map_gaussians.rs:26-79)
+            e_mx = q0.x; e_my = q0.y; e_conic.c00 = q0.z; e_conic.c01 = q0.w; e_conic.c11 = q1.x; e_pt = q3.x;
             float ex, ey;
-            bbox_extent(conic, pt, ex, ey);
-            bb = tile_bbox(mx, my, ex, ey, tiles_x, tiles_y);
-            e_mx = mx; e_my = my; e_conic = conic; e_pt = pt;
+            bbox_extent(e_conic, e_pt, ex, ey);
+            bb = tile_bbox(e_mx, e_my, ex, ey, tiles_x, tiles_y);
         }
         // pull the next ticket's rows towards L2 (the ids have arrived by now)
-        if (next_active) {
-            const char *srow = reinterpret_cast<const char *>(sh + (size_t)gid_next * KF);
-            const char *trow = reinterpret_cast<const char *>(transforms + (size_t)gid_next * 10);
-            if (VEC4) prefetch_l2_bulk(srow, KF * 4);
-            prefetch_l2_bulk(reinterpret_cast<const char *>(reinterpret_cast<uintptr_t>(trow) & ~(uintptr_t)15), 48);
-        }
+        if (next_active) prefetch_l2_bulk(row_by_gid + (size_t)gid_next * BG_PROJECTED_STRIDE, BG_PROJECTED_STRIDE * 4);
         // The output slots of a warp's 32 splats are one contiguous range [base(lane 0), end(last active lane)).
         const uint32_t warp_base = __shfl_sync(0xffffffffu, base, 0);
         uint32_t end_here = active ? base + budget : 0u;
@@ -565,20 +572,40 @@ tile_offsets_kernel(const uint32_t *__restrict__ tile_ids, const uint32_t *__res
 }
 
 // ---- host launchers (called from api.cu) ----
-cudaError_t launch_project_cull(cudaStream_t s, int grid, bool mip, const float *transforms, const float *raw_opac,
-                                uint32_t n, const BgCamera &u, uint32_t w, uint32_t h, uint32_t tx, uint32_t ty,
-                                uint32_t *depth_keys, uint32_t *gids, uint32_t *counts, float *max_radius,
-                                uint32_t *cgid_from_gid, unsigned long long *hit_masks, uint32_t *ctl,
-                                unsigned long long *lb, const uint32_t *epoch_base, uint32_t epoch_off) {
-    if (n == 0) return cudaSuccess;
+template <bool MIP>
+static cudaError_t launch_cull_deg(cudaStream_t s, int grid, int deg, const float *transforms, const float *sh,
+                                   const float *raw_opac, uint32_t n, const BgCamera &u, uint32_t w, uint32_t h,
+                                   uint32_t tx, uint32_t ty, uint32_t *depth_keys, uint32_t *gids, uint32_t *counts,
+                                   float *max_radius, uint32_t *cgid_from_gid, float *row_by_gid, uint32_t *ctl,
+                                   unsigned long long *lb, const uint32_t *epoch_base, uint32_t epoch_off) {
     const bool dist = u.camera_model != BG_CAMERA_PINHOLE;
-#define BG_LAUNCH_CULL(M, D)                                                                                       \
-    project_cull_kernel<M, D><<<grid, PROJ_THREADS, 0, s>>>(transforms, raw_opac, n, u, w, h, tx, ty, depth_keys, \
-                                                            gids, counts, max_radius, cgid_from_gid, hit_masks, ctl, lb, epoch_base, epoch_off)
-    if (mip) { if (dist) BG_LAUNCH_CULL(true, true); else BG_LAUNCH_CULL(true, false); }
-    else     { if (dist) BG_LAUNCH_CULL(false, true); else BG_LAUNCH_CULL(false, false); }
+#define BG_LAUNCH_CULL(D)                                                                                                  \
+    if (dist) project_cull_kernel<MIP, D, true><<<grid, PROJ_THREADS, 0, s>>>(transforms, sh, raw_opac, n, u, w, h, tx, ty, \
+                                       depth_keys, gids, counts, max_radius, cgid_from_gid, row_by_gid, ctl, lb, epoch_base, epoch_off); \
+    else project_cull_kernel<MIP, D, false><<<grid, PROJ_THREADS, 0, s>>>(transforms, sh, raw_opac, n, u, w, h, tx, ty,      \
+                                       depth_keys, gids, counts, max_radius, cgid_from_gid, row_by_gid, ctl, lb, epoch_base, epoch_off)
+    switch (deg) {
+        case 0: BG_LAUNCH_CULL(0); break;
+        case 1: BG_LAUNCH_CULL(1); break;
+        case 2: BG_LAUNCH_CULL(2); break;
+        case 3: BG_LAUNCH_CULL(3); break;
+        case 4: BG_LAUNCH_CULL(4); break;
+        default: return cudaErrorInvalidValue;
+    }
 #undef BG_LAUNCH_CULL
     return cudaGetLastError();
+}
+
+cudaError_t launch_project_cull(cudaStream_t s, int grid, bool mip, int deg, const float *transforms, const float *sh,
+                                const float *raw_opac, uint32_t n, const BgCamera &u, uint32_t w, uint32_t h,
+                                uint32_t tx, uint32_t ty, uint32_t *depth_keys, uint32_t *gids, uint32_t *counts,
+                                float *max_radius, uint32_t *cgid_from_gid, float *row_by_gid, uint32_t *ctl,
+                                unsigned long long *lb, const uint32_t *epoch_base, uint32_t epoch_off) {
+    if (n == 0) return cudaSuccess;
+    return mip ? launch_cull_deg<true>(s, grid, deg, transforms, sh, raw_opac, n, u, w, h, tx, ty, depth_keys, gids,
+                                       counts, max_radius, cgid_from_gid, row_by_gid, ctl, lb, epoch_base, epoch_off)
+               : launch_cull_deg<false>(s, grid, deg, transforms, sh, raw_opac, n, u, w, h, tx, ty, depth_keys, gids,
+                                        counts, max_radius, cgid_from_gid, row_by_gid, ctl, lb, epoch_base, epoch_off);
 }
 
 cudaError_t launch_gather_scan(cudaStream_t s, int grid, const uint32_t *in, const uint32_t *gather_idx,
@@ -591,41 +618,13 @@ cudaError_t launch_gather_scan(cudaStream_t s, int grid, const uint32_t *in, con
     return cudaGetLastError();
 }
 
-template <bool MIP>
-static cudaError_t launch_visible_deg(cudaStream_t s, int grid, int deg, const float *transforms, const float *sh,
-                                      const float *raw_opac, const uint32_t *gid_sorted, const uint32_t *cum,
-                                      const BgCamera &u, uint32_t tx, uint32_t ty, float *projected,
-                                      uint32_t *tile_keys, uint32_t *isect_vals, uint32_t cap,
-                                      uint32_t *cgid_from_gid, const unsigned long long *hit_masks, uint32_t *ctl,
-                                      uint32_t tile_bits) {
-    const bool dist = u.camera_model != BG_CAMERA_PINHOLE;
-#define BG_LAUNCH_VIS(D)                                                                                                   \
-    if (dist) project_visible_emit_kernel<MIP, D, true><<<grid, VIS_THREADS, 0, s>>>(transforms, sh, raw_opac, gid_sorted, cum, u, \
-                                                                     tx, ty, projected, tile_keys, isect_vals, cap, cgid_from_gid, hit_masks, ctl, tile_bits); \
-    else project_visible_emit_kernel<MIP, D, false><<<grid, VIS_THREADS, 0, s>>>(transforms, sh, raw_opac, gid_sorted, cum, u, \
-                                                                     tx, ty, projected, tile_keys, isect_vals, cap, cgid_from_gid, hit_masks, ctl, tile_bits)
-    switch (deg) {
-        case 0: BG_LAUNCH_VIS(0); break;
-        case 1: BG_LAUNCH_VIS(1); break;
-        case 2: BG_LAUNCH_VIS(2); break;
-        case 3: BG_LAUNCH_VIS(3); break;
-        case 4: BG_LAUNCH_VIS(4); break;
-        default: return cudaErrorInvalidValue;
-    }
-#undef BG_LAUNCH_VIS
+cudaError_t launch_project_visible_emit(cudaStream_t s, int grid, const float *row_by_gid, const uint32_t *gid_sorted,
+                                        const uint32_t *cum, uint32_t tx, uint32_t ty, float *projected,
+                                        uint32_t *tile_keys, uint32_t *isect_vals, uint32_t cap,
+                                        uint32_t *cgid_from_gid, uint32_t *ctl, uint32_t tile_bits) {
+    project_visible_emit_kernel<<<grid, VIS_THREADS, 0, s>>>(row_by_gid, gid_sorted, cum, tx, ty, projected, tile_keys,
+                                                             isect_vals, cap, cgid_from_gid, ctl, tile_bits);
     return cudaGetLastError();
-}
-
-cudaError_t launch_project_visible_emit(cudaStream_t s, int grid, bool mip, int deg, const float *transforms,
-                                        const float *sh, const float *raw_opac, const uint32_t *gid_sorted,
-                                        const uint32_t *cum, const BgCamera &u, uint32_t tx, uint32_t ty,
-                                        float *projected, uint32_t *tile_keys, uint32_t *isect_vals, uint32_t cap,
-                                        uint32_t *cgid_from_gid, const unsigned long long *hit_masks, uint32_t *ctl,
-                                        uint32_t tile_bits) {
-    return mip ? launch_visible_deg<true>(s, grid, deg, transforms, sh, raw_opac, gid_sorted, cum, u, tx, ty, projected,
-                                          tile_keys, isect_vals, cap, cgid_from_gid, hit_masks, ctl, tile_bits)
-               : launch_visible_deg<false>(s, grid, deg, transforms, sh, raw_opac, gid_sorted, cum, u, tx, ty,
-                                           projected, tile_keys, isect_vals, cap, cgid_from_gid, hit_masks, ctl, tile_bits);
 }
 
 cudaError_t launch_tile_offsets(cudaStream_t s, int grid, const uint32_t *tile_ids, const uint32_t *ctl,
