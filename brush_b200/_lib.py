@@ -16,7 +16,7 @@ BG_OK, BG_ERR_NULL, BG_ERR_INVALID, BG_ERR_CUDA, BG_ERR_CAPACITY, BG_ERR_UNSUPPO
 PASS_FORWARD, PASS_BACKWARD, PASS_BACKWARD_SMOOTH = 0, 1, 2
 PROJECTED_STRIDE = 16
 VCOMBINED_STRIDE = 10
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 _STATUS_NAMES = {1: "BG_ERR_NULL", 2: "BG_ERR_INVALID", 3: "BG_ERR_CUDA", 4: "BG_ERR_CAPACITY", 5: "BG_ERR_UNSUPPORTED"}
 
@@ -215,6 +215,8 @@ SIGNATURES = {
     "bg_dp_exchange": (_I32, [_P, _P, _P, _U32, _U32, _P, _P, _P, _P, _U32]),
     "bg_train_step_views_workspace_bytes": (_U64, [_U32, _U32, _U32, _U32, _U32, _U32]),
     "bg_train_step_views": (_I32, [_P, _P, _P, C.POINTER(BgTrainViewsArgs)]),
+    "bg_train_step_views_depth_workspace_bytes": (_U64, [_U32, _U32, _U32, _U32, _U32, _U32]),
+    "bg_train_step_views_depth": (_I32, [_P, _P, _P, C.POINTER(BgTrainViewsArgs), C.POINTER(BgDepthSupervision)]),
     "bg_refine_workspace_bytes": (_U64, [_U32]),
     "bg_refine": (_I32, [_P, _P, C.POINTER(BgRefineArgs), C.POINTER(BgRefineStats)]),
     "bg_bounds_percentile": (_I32, [_P, _P, _U32, _P, _F, _P, _U64, C.POINTER(_F)]),

@@ -1035,6 +1035,29 @@ ViewsWs carve_views_ws(void *base, uint32_t n, uint32_t k, uint32_t w, uint32_t 
     ws.bytes = off;
     return ws;
 }
+
+// the depth term's scratch of the multi-view step, behind the largest views workspace; reused view after view
+DepthWs carve_views_depth_ws(void *base, uint32_t n, uint32_t k, uint32_t w, uint32_t h, uint32_t local, uint32_t world) {
+    uint64_t off = carve_views_ws(nullptr, n, k, w, h, local, world, true).bytes;
+    auto take = [&](uint64_t floats) {
+        float *p = base ? reinterpret_cast<float *>(static_cast<char *>(base) + off) : nullptr;
+        off += (floats * 4 + 255) / 256 * 256;
+        return p;
+    };
+    DepthWs ws;
+    const uint64_t px = (uint64_t)w * h;
+    ws.depth = take(px);
+    ws.v_depth = take(px);
+    ws.v_z = take(std::max(n, 1u));
+    ws.partials = take(depth_loss_num_partials(h, w));
+    ws.bytes = off;
+    return ws;
+}
+
+// Whether view i of a multi-view depth step runs the depth term (DESIGN.md section 4.7).
+bool views_depth_term(const BgDepthSupervision *dep, uint32_t i) {
+    return dep && dep[i].weight > 0.0f && dep[i].valid_count > 0;
+}
 }  // namespace
 
 namespace bg {
@@ -1076,7 +1099,15 @@ extern "C" uint64_t bg_train_step_views_workspace_bytes(uint32_t n, uint32_t k, 
     return carve_views_ws(nullptr, n, k, w, h, std::max(local, 1u), std::max(world, 1u), true).bytes;
 }
 
-extern "C" int32_t bg_train_step_views(BgContext *c, BgDpComm *h, void *stream, BgTrainViewsArgs *a) {
+extern "C" uint64_t bg_train_step_views_depth_workspace_bytes(uint32_t n, uint32_t k, uint32_t w, uint32_t h, uint32_t local,
+                                                              uint32_t world) {
+    return carve_views_depth_ws(nullptr, n, k, w, h, std::max(local, 1u), std::max(world, 1u)).bytes;
+}
+
+// The multi-view step.  dep == nullptr: bg_train_step_views.  Otherwise dep[local_views] (validated by
+// bg_train_step_views_depth); a view whose term runs renders depth and folds its depth gradient into the exchange row, the
+// other views run exactly the plain view's launches.
+static int32_t train_step_views(BgContext *c, BgDpComm *h, void *stream, BgTrainViewsArgs *a, const BgDepthSupervision *dep) {
     if (!c || !a) return BG_ERR_NULL;
     if (!a->transforms || !a->sh || !a->raw_opac || !a->m_t || !a->v_t || !a->m_sh || !a->v_sh || !a->m_o || !a->v_o ||
         !a->refine_norm || !a->vis_weight || !a->max_screen || !a->cams || !a->gt_packed || !a->workspace || !a->loss_out)
@@ -1096,10 +1127,18 @@ extern "C" int32_t bg_train_step_views(BgContext *c, BgDpComm *h, void *stream, 
     const ViewsWs ws = carve_views_ws(a->workspace, n, k, w, hh, local, world, fold);
     if (ws.bytes > a->workspace_bytes) { set_err("bg_train_step_views: workspace too small (bg_train_step_views_workspace_bytes)", cudaSuccess); return BG_ERR_CAPACITY; }
     if (a->chunks > DP_MAX_CHUNKS) { set_err("bg_train_step_views: at most 16 chunks", cudaSuccess); return BG_ERR_INVALID; }
+    const DepthWs dws = carve_views_depth_ws(a->workspace, n, k, w, hh, local, world);
+    if (dep && dws.bytes > a->workspace_bytes) {
+        set_err("bg_train_step_views_depth: workspace too small (bg_train_step_views_depth_workspace_bytes)", cudaSuccess);
+        return BG_ERR_CAPACITY;
+    }
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
     const DpLayout L = dp_layout(n, local, world);
     int32_t r;
+    if (dep)
+        for (uint32_t i = 0; i < local; i++)
+            if (!views_depth_term(dep, i)) BG_CUDA(cudaMemsetAsync(dep[i].depth_loss_out, 0, sizeof(float), s));
     // the 3D-filter floor folded into what the renderer sees (bwd/burn_glue.rs:260-270)
     const float *r_t = a->transforms, *r_o = a->raw_opac;
     if (fold) {
@@ -1122,17 +1161,37 @@ extern "C" int32_t bg_train_step_views(BgContext *c, BgDpComm *h, void *stream, 
     // leave as soon as the last local view's blend backward is done and travel UNDER its projection backward; the summed
     // small rows and the MAX statistics (all-reduces) follow once that is done.  The update pass is split the same way:
     // the SH part (70 % of its traffic) needs the records only and runs under the all-reduces, the rest follows them.
+    bool alpha_dirty = false;   // a depth view added to v_output[...,3], which the 3-channel image loss leaves as it is
     for (uint32_t i = 0; i < local; i++) {
         const BgCamera *cam = a->cams + i;
-        r = bg_render_forward(c, stream, cam, w, hh, n, k, r_t, a->sh, r_o, a->mip, a->background, BG_PASS_BACKWARD, ws.out_img, ws.visible,
-                              ws.max_radius, &a->state_out);
+        const bool term = views_depth_term(dep, i);
+        if (alpha_dirty && a->channels == 3) BG_CUDA(cudaMemsetAsync(ws.v_output, 0, (size_t)w * hh * 4 * sizeof(float), s));
+        alpha_dirty = false;
+        if (term)
+            r = bg_render_forward_depth(c, stream, cam, w, hh, n, k, r_t, a->sh, r_o, a->mip, a->background, BG_PASS_BACKWARD, ws.out_img,
+                                        dws.depth, ws.visible, ws.max_radius, &a->state_out);
+        else
+            r = bg_render_forward(c, stream, cam, w, hh, n, k, r_t, a->sh, r_o, a->mip, a->background, BG_PASS_BACKWARD, ws.out_img,
+                                  ws.visible, ws.max_radius, &a->state_out);
         if (r != BG_OK) return r;
         r = bg_image_loss_fused(c, stream, ws.out_img, a->gt_packed[i], a->channels, hh, w, 1, (int64_t)w * 4, 4, a->l1_weight,
                                 a->ssim_weight, a->has_composite_bg ? a->composite_bg : nullptr, a->mask, chain, ws.v_output, ws.partials);
         if (r != BG_OK) return r;
         BG_CUDA(launch_loss_reduce(s, ws.partials, a->channels, bg_image_loss_num_partials(a->channels, hh, w) / a->channels, chain,
                                    ws.loss_terms + i));
-        r = bg_rasterize_backward(c, stream, &a->state_out, ws.out_img, ws.v_output, a->background, 0, ws.v_combined, n);
+        if (term) {
+            // the depth term: v_depth, v_output[...,3] += dL/da, L_d -> depth_loss_out and added to this view's loss term
+            const float dchain = dep[i].weight / (float)dep[i].valid_count;
+            r = bg_depth_loss_fused(c, stream, ws.out_img, dws.depth, dep[i].target, hh, w, dchain, ws.v_output, dws.v_depth, dws.partials);
+            if (r != BG_OK) return r;
+            BG_CUDA(launch_depth_loss_reduce(s, dws.partials, depth_loss_num_partials(hh, w), dchain, dep[i].depth_loss_out,
+                                             ws.loss_terms + i));
+            alpha_dirty = true;
+            r = bg_rasterize_backward_depth(c, stream, &a->state_out, ws.out_img, dws.depth, ws.v_output, dws.v_depth, a->background, 0,
+                                            ws.v_combined, n, dws.v_z);
+        } else {
+            r = bg_rasterize_backward(c, stream, &a->state_out, ws.out_img, ws.v_output, a->background, 0, ws.v_combined, n);
+        }
         if (r != BG_OK) return r;
         BG_CUDA(launch_pack_color(s, n, local, i, a->state_out.compact_from_global_gid, ws.v_combined, ws.record));
         if (d && i + 1 == local) {
@@ -1146,9 +1205,14 @@ extern "C" int32_t bg_train_step_views(BgContext *c, BgDpComm *h, void *stream, 
         }
         r = bg_project_backward_factored(c, stream, cam, &a->state_out, r_t, a->sh, r_o, ws.v_combined, ws.v_t, ws.v_color, ws.v_o, ws.v_refine);
         if (r != BG_OK) return r;
-        // fold the view into the exchange rows (sum of the small gradients, MAX statistics)
-        BG_CUDA(launch_pack_view(s, n, local, i, i == 0, ws.v_t, ws.v_o, nullptr, ws.v_refine, ws.visible, ws.max_radius, ws.small, ws.stat,
-                                 ws.record));
+        // fold the view into the exchange rows (sum of the small gradients, MAX statistics); a depth view also folds in
+        // its mean gradient v_z * R[2,:] on the way (the rounding of depth_to_means, no pass of its own)
+        if (term)
+            BG_CUDA(launch_pack_view_depth(s, n, local, i, i == 0, ws.v_t, ws.v_o, ws.v_refine, ws.visible, ws.max_radius,
+                                           a->state_out.compact_from_global_gid, dws.v_z, *cam, ws.small, ws.stat, ws.record));
+        else
+            BG_CUDA(launch_pack_view(s, n, local, i, i == 0, ws.v_t, ws.v_o, nullptr, ws.v_refine, ws.visible, ws.max_radius, ws.small,
+                                     ws.stat, ws.record));
     }
     BG_CUDA(launch_loss_mean(s, ws.loss_terms, local, a->loss_out));
     UpdateParams P;
@@ -1192,6 +1256,32 @@ extern "C" int32_t bg_train_step_views(BgContext *c, BgDpComm *h, void *stream, 
     tr.mark(6, s);
     tr.report(s, d->stream, d->rank);
     return BG_OK;
+}
+
+extern "C" int32_t bg_train_step_views(BgContext *c, BgDpComm *h, void *stream, BgTrainViewsArgs *a) {
+    return train_step_views(c, h, stream, a, nullptr);
+}
+
+// ---- bg_train_step_views_depth: bg_train_step_views with the depth term of DESIGN.md section 4.7 on the views that carry one.
+// The depth gradient reaches v_transforms[:, 0:3] and the refine weight only, both already in the exchanged rows: the
+// exchange is unchanged, and ranks with and without depth views share a step.
+extern "C" int32_t bg_train_step_views_depth(BgContext *c, BgDpComm *h, void *stream, BgTrainViewsArgs *a, const BgDepthSupervision *depth) {
+    if (!c || !a || !depth) return BG_ERR_NULL;
+    const uint32_t local = a->local_views;
+    if (local == 0 || local > DP_MAX_VIEWS) { set_err("bg_train_step_views_depth: 1..16 views per step in total", cudaSuccess); return BG_ERR_INVALID; }
+    for (uint32_t i = 0; i < local; i++) {
+        if (!depth[i].depth_loss_out) return BG_ERR_NULL;
+        if (!(depth[i].weight >= 0.0f) || !std::isfinite(depth[i].weight)) {
+            set_err("bg_train_step_views_depth: weight must be finite and >= 0", cudaSuccess);
+            return BG_ERR_INVALID;
+        }
+        if (views_depth_term(depth, i) && !depth[i].target) return BG_ERR_NULL;
+        if (views_depth_term(depth, i) && (uintptr_t)depth[i].target % 4) {
+            set_err("bg_train_step_views_depth: target must be 4-byte aligned", cudaSuccess);
+            return BG_ERR_INVALID;
+        }
+    }
+    return train_step_views(c, h, stream, a, depth);
 }
 
 // ---- refine (refine.cu): every decision on the device, one readback of the counts at the end

@@ -58,6 +58,10 @@ cudaError_t launch_write_header(cudaStream_t s, float *hdr, const DpHeader &h, u
 cudaError_t launch_pack_view(cudaStream_t s, uint32_t n, uint32_t local, uint32_t li, bool first, const float *v_t, const float *v_o,
                              const float *v_color, const float *v_refine, const float *visible, const float *max_radius, float *small,
                              float *stat, float *record);
+// launch_pack_view with the depth term's mean gradient v_z * R[2,:] folded into v_transforms[0:3] (no colour record)
+cudaError_t launch_pack_view_depth(cudaStream_t s, uint32_t n, uint32_t local, uint32_t li, bool first, const float *v_t, const float *v_o,
+                                   const float *v_refine, const float *visible, const float *max_radius, const uint32_t *cgid_from_gid,
+                                   const float *v_z, const BgCamera &cam, float *small, float *stat, float *record);
 cudaError_t launch_pack_color(cudaStream_t s, uint32_t n, uint32_t local, uint32_t li, const uint32_t *cgid_from_gid,
                               const float *v_combined, float *record);
 

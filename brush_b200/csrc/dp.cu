@@ -195,16 +195,31 @@ __global__ void write_header_kernel(float *hdr, DpHeader h, uint32_t local) {
 // Folds one local view's gradients into the exchange buffers: small row (+)= (v_transforms, v_raw_opac, visible), the stat
 // row keeps the running MAX of the refine weight / radius (stats.rs:40-50 over the rank's views), the record row gets the
 // view's colour gradient.  The first view assigns, the others accumulate.
+// DEPTH: the view also carries the depth term's v_z (bg_rasterize_backward_depth, indexed by compact id); its mean
+// gradient v_z * R[2,:] is folded into the row's v_transforms[0:3] before the sum, with the rounding and the skip rules of
+// depth_to_means_kernel (project_bwd.cu: multiply, then add; a culled Gaussian or a zero v_z leaves the bits alone), so
+// the row equals depth_to_means followed by the plain pack bit for bit -- without a read-modify-write pass over v_t.
+template <bool DEPTH>
 __global__ void __launch_bounds__(256)
 pack_view_kernel(uint32_t n, uint32_t rec_row, uint32_t li, int first, const float *__restrict__ v_t, const float *__restrict__ v_o,
                  const float *__restrict__ v_color, const float *__restrict__ v_refine, const float *__restrict__ visible,
-                 const float *__restrict__ max_radius, float *__restrict__ small, float *__restrict__ stat, float *__restrict__ record) {
+                 const float *__restrict__ max_radius, float *__restrict__ small, float *__restrict__ stat, float *__restrict__ record,
+                 const uint32_t *__restrict__ cgid_from_gid, const float *__restrict__ v_z, float r0, float r1, float r2) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     float row[DP_SMALL_ROW];
     const float2 *t2 = reinterpret_cast<const float2 *>(v_t + (size_t)i * 10);
 #pragma unroll
     for (int q = 0; q < 5; q++) { const float2 a = __ldg(t2 + q); row[2 * q] = a.x; row[2 * q + 1] = a.y; }
+    if constexpr (DEPTH) {
+        const uint32_t cg = __ldg(cgid_from_gid + i);
+        const float vz = cg != 0xFFFFFFFFu ? __ldg(v_z + cg) : 0.0f;
+        if (vz != 0.0f) {
+            row[0] = __fadd_rn(row[0], __fmul_rn(vz, r0));
+            row[1] = __fadd_rn(row[1], __fmul_rn(vz, r1));
+            row[2] = __fadd_rn(row[2], __fmul_rn(vz, r2));
+        }
+    }
     row[10] = __ldg(v_o + i);
     row[11] = __ldg(visible + i);
     float4 *dst = reinterpret_cast<float4 *>(small + (size_t)i * DP_SMALL_ROW);
@@ -262,8 +277,17 @@ cudaError_t launch_pack_view(cudaStream_t s, uint32_t n, uint32_t local, uint32_
                              const float *v_color, const float *v_refine, const float *visible, const float *max_radius, float *small,
                              float *stat, float *record) {
     if (n == 0) return cudaSuccess;
-    pack_view_kernel<<<(n + 255) / 256, 256, 0, s>>>(n, 3 * local, li, first ? 1 : 0, v_t, v_o, v_color, v_refine, visible, max_radius,
-                                                     small, stat, record);
+    pack_view_kernel<false><<<(n + 255) / 256, 256, 0, s>>>(n, 3 * local, li, first ? 1 : 0, v_t, v_o, v_color, v_refine, visible,
+                                                            max_radius, small, stat, record, nullptr, nullptr, 0.0f, 0.0f, 0.0f);
+    return cudaGetLastError();
+}
+cudaError_t launch_pack_view_depth(cudaStream_t s, uint32_t n, uint32_t local, uint32_t li, bool first, const float *v_t, const float *v_o,
+                                   const float *v_refine, const float *visible, const float *max_radius, const uint32_t *cgid_from_gid,
+                                   const float *v_z, const BgCamera &cam, float *small, float *stat, float *record) {
+    if (n == 0) return cudaSuccess;
+    pack_view_kernel<true><<<(n + 255) / 256, 256, 0, s>>>(n, 3 * local, li, first ? 1 : 0, v_t, v_o, nullptr, v_refine, visible,
+                                                           max_radius, small, stat, record, cgid_from_gid, v_z, cam.viewmat[2],
+                                                           cam.viewmat[5], cam.viewmat[8]);
     return cudaGetLastError();
 }
 

@@ -230,6 +230,7 @@ class TrainStepStats:
     lr_mean: float
     loss: torch.Tensor  # lazy device scalar (msg.rs:16-27); image loss + depth loss
     depth_loss: Optional[torch.Tensor] = None   # the depth term alone (None when the batch carries no depth)
+    view_depth_losses: Optional[torch.Tensor] = None   # step_views_depth: device [local views], each view's depth term
 
 
 class SplatTrainer:
@@ -253,6 +254,7 @@ class SplatTrainer:
         self._views_buf = None
         self._views_ws = None
         self._views_loss = None
+        self._views_depth_loss = None
         self._dp_comm = None
         self._dp_group = None
         self._fused_ws = None
@@ -474,20 +476,48 @@ class SplatTrainer:
         own NCCL communicator (all-reduce SUM 48 N B, all-reduce MAX 8 N B, all-gather 12 local N B per rank), runs the SH
         part of the update pass under the all-reduces, and all ranks apply bit-identical updates.  At most 16 views per step in total.  All views of a
         step share the image size and the loss configuration.  distributed=False runs the step on this device alone even
-        inside an initialised process group."""
+        inside an initialised process group.  Views with depth and a positive depth_loss_weight go through
+        step_views_depth."""
+        return self._step_views(batches, splats, group, chunks, distributed, with_depth=False)
+
+    def step_views_depth(self, batches: Sequence[SceneBatch], splats: Splats, group=None, chunks: int = 0,
+                         distributed: Optional[bool] = None) -> TrainStepStats:
+        """step_views with depth supervision (DESIGN.md section 4.7) through ONE ABI call (bg_train_step_views_depth):
+        every batch may carry depth / depth_count, and each view whose map has valid pixels adds its depth term with
+        TrainConfig.depth_loss_weight.  The views and rank rules are those of step_views; ranks with and without depth
+        views share a step (the exchange is the same).  loss is the mean over this rank's views of image + depth loss,
+        depth_loss the mean of the views' depth terms and view_depth_losses each view's term, all on the device (views of
+        buffers the next step overwrites).  With depth_loss_weight == 0 or no batch carrying depth this is step_views
+        with a zero depth_loss."""
+        cfg = self.config
+        if cfg.depth_loss_weight == 0.0 or all(b.depth is None for b in batches):
+            st = self._step_views(batches, splats, group, chunks, distributed, with_depth=False)
+            zeros = torch.zeros(len(batches), dtype=torch.float32, device=self.ctx.device)
+            st.depth_loss, st.view_depth_losses = zeros.sum(), zeros
+            return st
+        return self._step_views(batches, splats, group, chunks, distributed, with_depth=True)
+
+    def _step_views(self, batches, splats, group, chunks, distributed, with_depth: bool) -> TrainStepStats:
         import torch.distributed as dist
         cfg = self.config
         self._ensure_state(splats)
-        st = self._state
         dev = self.ctx.device
         lib = _lib.load()
         multi = dist.is_initialized() and dist.get_world_size(group) > 1 if distributed is None else bool(distributed)
         world = dist.get_world_size(group) if multi else 1
         local = len(batches)
+        who = "step_views_depth" if with_depth else "step_views"
         if local == 0 or local * world > 16:
-            raise ValueError("step_views needs 1..16 views per step in total")
-        if cfg.depth_loss_weight > 0.0 and any(b.depth is not None for b in batches):
-            raise ValueError("step_views has no depth term: train views with depth through step() or step_fused()")
+            raise ValueError(f"{who} needs 1..16 views per step in total")
+        if not with_depth and cfg.depth_loss_weight > 0.0 and any(b.depth is not None for b in batches):
+            raise ValueError("step_views has no depth term: train views with depth through step_views_depth(), step() or "
+                             "step_fused()")
+        # depth maps checked and the targets on the device before anything runs
+        if with_depth:
+            for b in batches:
+                if b.depth is not None and tuple(b.depth.shape) != b.img_size():
+                    raise ValueError(f"SceneBatch.depth must be [{b.img_size()[0]},{b.img_size()[1]}], got {tuple(b.depth.shape)}")
+        targets = [self._depth_target(b) if with_depth and self._depth_term(b) else None for b in batches]
         if multi and (self._dp_comm is None or self._dp_group is not group):
             from .dp import DpComm
             self._dp_comm, self._dp_group = DpComm(self.ctx, group), group
@@ -498,10 +528,45 @@ class SplatTrainer:
         for b in batches:
             if b.img_size() != (img_h, img_w) or (b.has_alpha, b.masked_alpha) != (b0.has_alpha, b0.masked_alpha):
                 raise ValueError("the views of one step must share the image size and the alpha mode")
-        need = int(lib.bg_train_step_views_workspace_bytes(n, k, img_w, img_h, local, world))
+        ws_bytes = lib.bg_train_step_views_depth_workspace_bytes if with_depth else lib.bg_train_step_views_workspace_bytes
+        need = int(ws_bytes(n, k, img_w, img_h, local, world))
         if self._views_ws is None or self._views_ws.numel() < need:
             self._views_ws = torch.empty(need, dtype=torch.uint8, device=dev)
             self._views_loss = torch.zeros(1, dtype=torch.float32, device=dev)
+        a, lr_mean, keep = self._views_args(batches, splats, self._views_ws, need, chunks)
+        a.loss_out = self._views_loss.data_ptr()
+        comm = self._dp_comm.handle if multi else None
+        if not with_depth:
+            _lib.check(lib.bg_train_step_views(self.ctx.handle, comm, _stream_ptr(dev), C.byref(a)), "bg_train_step_views")
+            self._views_keepalive = keep
+            return TrainStepStats(num_visible_event=None, lr_mean=lr_mean, loss=self._views_loss[0])
+        if self._views_depth_loss is None:
+            self._views_depth_loss = torch.zeros(16, dtype=torch.float32, device=dev)
+        ds = self._views_depth_args(batches, targets, self._views_depth_loss)
+        _lib.check(lib.bg_train_step_views_depth(self.ctx.handle, comm, _stream_ptr(dev), C.byref(a), ds), "bg_train_step_views_depth")
+        self._views_keepalive = (keep, targets, ds)
+        per_view = self._views_depth_loss[:local]
+        return TrainStepStats(num_visible_event=None, lr_mean=lr_mean, loss=self._views_loss[0], depth_loss=per_view.mean(),
+                              view_depth_losses=per_view)
+
+    def _views_depth_args(self, batches, targets, losses: torch.Tensor):
+        """The host array of BgDepthSupervision of step_views_depth: one per view, view i's depth loss into losses[i]."""
+        ds = (_lib.BgDepthSupervision * len(batches))()
+        for i, (b, t) in enumerate(zip(batches, targets)):
+            ds[i].target = t.data_ptr() if t is not None else None
+            ds[i].weight = float(self.config.depth_loss_weight)
+            ds[i].valid_count = int(b.depth_count) if b.depth is not None else 0
+            ds[i].depth_loss_out = losses.data_ptr() + 4 * i
+        return ds
+
+    def _views_args(self, batches, splats, ws, need, chunks):
+        """BgTrainViewsArgs of step_views for the current step_count (loss_out left unset); also returns the learning rate
+        and the host objects the arguments point into, which must outlive the call."""
+        cfg, st, dev = self.config, self._state, self.ctx.device
+        n, k = splats.num_splats(), splats.sh_coeffs.shape[1]
+        img_h, img_w = batches[0].img_size()
+        b0 = batches[0]
+        local = len(batches)
         from .camera import build_uniforms
         background = self.sample_background()          # shared seed: identical on every rank
         median_scale = self.bounds.median_size()
@@ -528,12 +593,8 @@ class SplatTrainer:
         a.lr_coeffs_dc, a.lr_coeffs_sh_scale, a.lr_opac = cfg.lr_coeffs_dc, cfg.lr_coeffs_sh_scale, cfg.lr_opac
         a.noise_scale = float(np.float32(lr_mean) * np.float32(cfg.mean_noise_weight))
         a.median_scale, a.seed, a.step, a.chunks = float(median_scale), int(cfg.seed), self.step_count, int(chunks)
-        a.workspace, a.workspace_bytes = self._views_ws.data_ptr(), need
-        a.loss_out = self._views_loss.data_ptr()
-        comm = self._dp_comm.handle if multi else None
-        _lib.check(lib.bg_train_step_views(self.ctx.handle, comm, _stream_ptr(dev), C.byref(a)), "bg_train_step_views")
-        self._views_keepalive = (gts, cams, ptrs)
-        return TrainStepStats(num_visible_event=None, lr_mean=lr_mean, loss=self._views_loss[0])
+        a.workspace, a.workspace_bytes = ws.data_ptr(), need
+        return a, lr_mean, (gts, cams, ptrs)
 
     def _apply_updates(self, splats, v_t, v_sh, v_o, v_r, visible, max_radius, median_scale) -> float:
         """Adam on the three parameter tensors, refine statistics, mean noise (train.rs:300-416): ONE pass over the

@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define BG_ABI_VERSION 7u
+#define BG_ABI_VERSION 8u
 
 /* f32 lanes per projected splat: a 64-byte row, four aligned 128-bit loads.  Lanes 0..8 are the reference
  * layout (kernels/helpers.rs:49-53: xy_x, xy_y, conic_x, conic_y, conic_z, color_a, color_r, color_g, color_b).
@@ -448,6 +448,22 @@ typedef struct {
 uint64_t bg_train_step_views_workspace_bytes(uint32_t n, uint32_t k, uint32_t w, uint32_t h, uint32_t local_views,
                                              uint32_t world);
 int32_t bg_train_step_views(BgContext *ctx, BgDpComm *comm, void *stream, BgTrainViewsArgs *args);
+
+/* bg_train_step_views with depth supervision (DESIGN.md section 4.7): depth is a host array of local_views entries, one per
+ * local view.  View i runs the term when depth[i].weight > 0 and depth[i].valid_count > 0: bg_render_forward_depth -> image
+ * loss -> bg_depth_loss_fused (chain = weight / valid_count) -> L_d,i into depth[i].depth_loss_out and added to the view's
+ * loss -> bg_rasterize_backward_depth -> the colour record -> bg_project_backward_factored -> the exchange row with v_z R[2,:]
+ * folded into v_transforms[0:3] (the rounding of bg_project_backward_depth).  Any other view runs the plain view's
+ * launches and gets 0 in its depth_loss_out; with no term on any local view the step runs the launches of
+ * bg_train_step_views.  *loss_out = mean over this rank's views of (image loss + L_d,i); the gradient is the mean over all
+ * views of the bg_train_step_depth gradients.  The depth gradient lives in the rows the exchange already carries, so ranks
+ * with and without depth views share a step.  workspace: bg_train_step_views_depth_workspace_bytes (else
+ * BG_ERR_CAPACITY).  Checked before the first launch: null depth, a null depth_loss_out or a null target on a view whose term
+ * runs is BG_ERR_NULL; a negative or non-finite weight is BG_ERR_INVALID; every check of bg_train_step_views applies. */
+uint64_t bg_train_step_views_depth_workspace_bytes(uint32_t n, uint32_t k, uint32_t w, uint32_t h, uint32_t local_views,
+                                                   uint32_t world);
+int32_t bg_train_step_views_depth(BgContext *ctx, BgDpComm *comm, void *stream, BgTrainViewsArgs *args,
+                                  const BgDepthSupervision *depth /* host [local_views] */);
 
 /* Building blocks of the exchange for hosts that drive the operators themselves.  The SH part of the
  * gradient of ONE view is rank one per Gaussian: v_sh[g,k,:] = Y_k(dir(mean_g, camera)) * v_color[g,:]

@@ -618,14 +618,54 @@ class SplatTrainer {
     const float *step_views(Context &ctx, DpComm *comm, cudaStream_t stream, const std::vector<Camera> &cameras,
                             const std::vector<const uint32_t *> &gt_packed, uint32_t w, uint32_t h, Splats &splats,
                             const float *min_scale = nullptr, bool has_alpha = false, bool masked_alpha = false) {
+        std::vector<BgCamera> cams;
+        BgTrainViewsArgs a = views_args(comm, cameras, gt_packed, w, h, splats, min_scale, has_alpha, masked_alpha, cams, false);
+        check(bg_train_step_views(ctx.handle(), comm ? comm->handle() : nullptr, stream, &a), "SplatTrainer::step_views");
+        last_state_ = a.state_out;
+        return loss_.data();
+    }
+    // step_views with depth supervision (bg_train_step_views_depth, DESIGN.md section 4.7): depth_targets[i] is camera i's
+    // device [h,w] metric camera-space z (0 = no measurement) or null, depth_valid_counts[i] its number of valid pixels
+    // (0 for none).  Each view whose map has valid pixels adds its depth term with cfg.depth_loss_weight.  Returns the
+    // device scalar of the loss (mean over this rank's views of image + depth loss) and the device float[local] of the
+    // views' depth losses.
+    struct ViewsLosses {
+        const float *loss;
+        const float *depth_losses;
+    };
+    ViewsLosses step_views(Context &ctx, DpComm *comm, cudaStream_t stream, const std::vector<Camera> &cameras,
+                           const std::vector<const uint32_t *> &gt_packed, const std::vector<const float *> &depth_targets,
+                           const std::vector<uint32_t> &depth_valid_counts, uint32_t w, uint32_t h, Splats &splats,
+                           const float *min_scale = nullptr, bool has_alpha = false, bool masked_alpha = false) {
+        if (depth_targets.size() != cameras.size() || depth_valid_counts.size() != cameras.size())
+            throw Error(BG_ERR_INVALID, "SplatTrainer::step_views: one depth target and valid count per camera");
+        std::vector<BgCamera> cams;
+        BgTrainViewsArgs a = views_args(comm, cameras, gt_packed, w, h, splats, min_scale, has_alpha, masked_alpha, cams, true);
+        std::vector<BgDepthSupervision> d(cameras.size());
+        for (size_t i = 0; i < d.size(); i++) {
+            d[i].target = depth_targets[i];
+            d[i].weight = cfg_.depth_loss_weight;
+            d[i].valid_count = depth_targets[i] ? depth_valid_counts[i] : 0u;
+            d[i].depth_loss_out = views_depth_loss_.data() + i;
+        }
+        check(bg_train_step_views_depth(ctx.handle(), comm ? comm->handle() : nullptr, stream, &a, d.data()), "SplatTrainer::step_views (depth)");
+        last_state_ = a.state_out;
+        return {loss_.data(), views_depth_loss_.data()};
+    }
+
+   private:
+    BgTrainViewsArgs views_args(DpComm *comm, const std::vector<Camera> &cameras, const std::vector<const uint32_t *> &gt_packed,
+                                uint32_t w, uint32_t h, Splats &splats, const float *min_scale, bool has_alpha, bool masked_alpha,
+                                std::vector<BgCamera> &cams, bool depth) {
         const uint32_t local = (uint32_t)cameras.size(), world = comm ? (uint32_t)comm->world() : 1u;
         if (local == 0 || gt_packed.size() != cameras.size() || local * world > 16)
             throw Error(BG_ERR_INVALID, "SplatTrainer::step_views: 1..16 views per step in total, one image per camera");
         if (splats.n != n_ || splats.k != k_) throw Error(BG_ERR_INVALID, "SplatTrainer::step_views: splat count differs from the optimizer state");
         step_ += 1;
-        const uint64_t need = bg_train_step_views_workspace_bytes(n_, k_, w, h, local, world);
+        const uint64_t need = depth ? bg_train_step_views_depth_workspace_bytes(n_, k_, w, h, local, world)
+                                    : bg_train_step_views_workspace_bytes(n_, k_, w, h, local, world);
         if (views_ws_.size() < need) views_ws_ = DeviceBuffer<unsigned char>(need);
-        std::vector<BgCamera> cams(local);
+        cams.resize(local);
         for (uint32_t i = 0; i < local; i++) cams[i] = make_uniforms(cameras[i], w, h);
         BgTrainViewsArgs a;
         std::memset(&a, 0, sizeof(a));
@@ -658,10 +698,10 @@ class SplatTrainer {
         a.chunks = 0;
         a.workspace = views_ws_.data(); a.workspace_bytes = need;
         a.loss_out = loss_.data();
-        check(bg_train_step_views(ctx.handle(), comm ? comm->handle() : nullptr, stream, &a), "SplatTrainer::step_views");
-        last_state_ = a.state_out;
-        return loss_.data();
+        return a;
     }
+
+   public:
 
     // SplatTrainer::refine + refine_splats + prune_points (train.rs:431-893) through bg_refine: every decision on the
     // device, one readback of the counts.  Replaces the tensors of `splats` and the optimizer state (the count changes),
@@ -734,7 +774,7 @@ class SplatTrainer {
     double decay_ = 1.0;
     int step_ = 0;
     DeviceBuffer<float> m_t_, v_t_, m_sh_, v_sh_, m_o_, v_o_, refine_norm_, vis_weight_, max_screen_, loss_;
-    DeviceBuffer<float> depth_loss_{1, true};
+    DeviceBuffer<float> depth_loss_{1, true}, views_depth_loss_{16, true};
     DeviceBuffer<unsigned char> ws_, views_ws_;
     BgRenderState last_state_{};
     BoundingBox bounds_;
