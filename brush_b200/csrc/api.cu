@@ -50,7 +50,6 @@ cudaError_t launch_project_bwd(cudaStream_t, bool, int, const float *, const flo
                                float *, float *);
 cudaError_t launch_depth_to_means(cudaStream_t, const uint32_t *, const float *, uint32_t, const BgCamera &, float *);
 cudaError_t launch_normal_noise(cudaStream_t, uint64_t, uint64_t, uint64_t, float *);
-cudaError_t launch_train_fill_lr(cudaStream_t, float *, float *, uint32_t, float, float, float, float);
 cudaError_t launch_loss_reduce(cudaStream_t, const float *, uint32_t, uint32_t, const float *, float *);
 cudaError_t launch_min_scale(cudaStream_t, uint32_t, const float *, const float *, uint32_t, float, float *);
 cudaError_t launch_fold_min_scale_fwd(cudaStream_t, uint32_t, const float *, const float *, const float *, float *, float *);
@@ -692,21 +691,30 @@ extern "C" int32_t bg_normal_noise(BgContext *c, void *stream, uint64_t seed, ui
     return BG_OK;
 }
 
-// compiler-rt __powisf2 is defined above (powi_f32).  Fills the step-dependent constants of the update pass.
-static void fill_update_consts(UpdateParams &P, float lr_mean, float lr_rotation, float lr_scale, float lr_coeffs_dc,
-                               float lr_coeffs_sh_scale, float lr_opac, float noise_scale, float median_scale, uint64_t seed,
-                               int32_t step, uint32_t n) {
-    for (int i = 0; i < 10; i++) P.lr_t[i] = i < 3 ? lr_mean : (i < 7 ? lr_rotation : lr_scale);   // train.rs:328-350
-    P.lr_sh_dc = 1.0f * lr_coeffs_dc;                                   // lr_scale_per_col * lr, as AdamScaled forms it
-    P.lr_sh_rest = (1.0f / lr_coeffs_sh_scale) * lr_coeffs_dc;
-    P.lr_opac = lr_opac;
+// The update pass over all n Gaussians of `a` (BgTrainUpdateArgs, BgTrainStepArgs or BgTrainViewsArgs, which name the
+// trainable state and the schedule alike): the state pointers and the step-dependent constants, unit gradient scales.
+// The caller sets the gradient sources.  compiler-rt __powisf2 is defined above (powi_f32).
+template <class A>
+static UpdateParams update_params(const A *a) {
+    UpdateParams P;
+    memset(&P, 0, sizeof(P));
+    P.g_begin = 0; P.count = a->n;
+    P.transforms = a->transforms; P.sh = a->sh; P.raw_opac = a->raw_opac;
+    P.m_t = a->m_t; P.v_t = a->v_t; P.m_sh = a->m_sh; P.v_sh = a->v_sh; P.m_o = a->m_o; P.v_o = a->v_o;
+    P.refine_norm = a->refine_norm; P.vis_weight = a->vis_weight; P.max_screen = a->max_screen;
+    P.grad_scale = 1.0f; P.sh_grad_scale = 1.0f;
+    for (int i = 0; i < 10; i++) P.lr_t[i] = i < 3 ? a->lr_mean : (i < 7 ? a->lr_rotation : a->lr_scale);   // train.rs:328-350
+    P.lr_sh_dc = 1.0f * a->lr_coeffs_dc;                                // lr_scale_per_col * lr, as AdamScaled forms it
+    P.lr_sh_rest = (1.0f / a->lr_coeffs_sh_scale) * a->lr_coeffs_dc;
+    P.lr_opac = a->lr_opac;
     P.beta1 = 0.9f; P.beta2 = 0.999f; P.eps = 1e-15f; P.f1 = 1.0f - P.beta1; P.f2 = 1.0f - P.beta2;
-    P.inv_bc1 = 1.0f / (1.0f - powi_f32(P.beta1, step)); P.inv_bc2 = 1.0f / (1.0f - powi_f32(P.beta2, step));
-    P.first = step == 1;
-    P.noisy = noise_scale != 0.0f;
-    P.noise_scale = noise_scale; P.median_scale = median_scale;
-    P.seed = seed;
-    P.noise_offset = (unsigned long long)(step - 1) * (((unsigned long long)n * 3 + 3) / 4);
+    P.inv_bc1 = 1.0f / (1.0f - powi_f32(P.beta1, a->step)); P.inv_bc2 = 1.0f / (1.0f - powi_f32(P.beta2, a->step));
+    P.first = a->step == 1;
+    P.noisy = a->noise_scale != 0.0f;
+    P.noise_scale = a->noise_scale; P.median_scale = a->median_scale;
+    P.seed = a->seed;
+    P.noise_offset = (unsigned long long)(a->step - 1) * (((unsigned long long)a->n * 3 + 3) / 4);
+    return P;
 }
 
 extern "C" int32_t bg_train_update(BgContext *c, void *stream, const BgTrainUpdateArgs *a) {
@@ -720,17 +728,9 @@ extern "C" int32_t bg_train_update(BgContext *c, void *stream, const BgTrainUpda
     if (deg < 0) { set_err("Invalid nr. of sh bases", cudaSuccess); return BG_ERR_INVALID; }
     if (a->step < 1) { set_err("bg_train_update: step is 1-based", cudaSuccess); return BG_ERR_INVALID; }
     BG_CUDA(cudaSetDevice(c->device));
-    UpdateParams P;
-    memset(&P, 0, sizeof(P));
-    P.g_begin = 0; P.count = a->n;
-    P.transforms = a->transforms; P.sh = a->sh; P.raw_opac = a->raw_opac;
-    P.m_t = a->m_t; P.v_t = a->v_t; P.m_sh = a->m_sh; P.v_sh = a->v_sh; P.m_o = a->m_o; P.v_o = a->v_o;
-    P.refine_norm = a->refine_norm; P.vis_weight = a->vis_weight; P.max_screen = a->max_screen;
+    UpdateParams P = update_params(a);
     P.g_t = a->v_transforms; P.g_o = a->v_raw_opac; P.g_sh = a->v_sh_grad;
-    P.grad_scale = 1.0f; P.sh_grad_scale = 1.0f;
     P.v_refine = a->v_refine; P.max_radius = a->max_radius; P.visible = a->visible;
-    fill_update_consts(P, a->lr_mean, a->lr_rotation, a->lr_scale, a->lr_coeffs_dc, a->lr_coeffs_sh_scale, a->lr_opac,
-                       a->noise_scale, a->median_scale, a->seed, a->step, a->n);
     BG_CUDA(launch_train_update((cudaStream_t)stream, deg, P, false));
     return BG_OK;
 }
@@ -738,60 +738,62 @@ extern "C" int32_t bg_train_update(BgContext *c, void *stream, const BgTrainUpda
 // ---- bg_train_step: SplatTrainer::step (brush-train/src/train.rs:176-429) as ONE call: every launch of the step on
 // the caller's stream, nothing read back, scratch from a caller-provided workspace.
 namespace {
+// Bump allocator over a workspace: take<T>(count) returns the next count elements and rounds the block up to 256 bytes.
+// base == nullptr only sizes the workspace: off ends as its byte count.
+struct Carver {
+    void *base;
+    uint64_t off = 0;
+    template <class T = float>
+    T *take(uint64_t count) {
+        T *p = base ? reinterpret_cast<T *>(static_cast<char *>(base) + off) : nullptr;
+        off += (count * sizeof(T) + 255) / 256 * 256;
+        return p;
+    }
+};
+
 struct TrainWs {
-    float *out_img, *v_output, *partials, *v_combined, *v_t, *v_sh, *v_o, *v_r, *visible, *max_radius, *noise, *t_lr, *sh_scale;
+    float *out_img, *v_output, *partials, *v_combined, *v_t, *v_sh, *v_o, *v_r, *visible, *max_radius;
     uint64_t bytes;
 };
 TrainWs carve_train_ws(void *base, uint32_t n, uint32_t k, uint32_t w, uint32_t h, uint32_t channels) {
-    uint64_t off = 0;
-    auto take = [&](uint64_t floats) {
-        float *p = base ? reinterpret_cast<float *>(static_cast<char *>(base) + off) : nullptr;
-        off += (floats * 4 + 255) / 256 * 256;
-        return p;
-    };
+    Carver cv{base};
     TrainWs ws;
     const uint64_t px = (uint64_t)w * h;
-    ws.out_img = take(px * 4);
-    ws.v_output = take(px * 4);
-    ws.partials = take(bg_image_loss_num_partials(channels, h, w));
-    ws.v_combined = take((uint64_t)n * BG_VCOMBINED_STRIDE);
-    ws.v_t = take((uint64_t)n * 10);
-    ws.v_sh = take((uint64_t)n * k * 3);
-    ws.v_o = take(n);
-    ws.v_r = take(n);
-    ws.visible = take(n);
-    ws.max_radius = take(n);
-    ws.noise = take((uint64_t)n * 3);
-    ws.t_lr = take(16);
-    ws.sh_scale = take((uint64_t)k * 3);
-    ws.bytes = off;
+    ws.out_img = cv.take(px * 4);
+    ws.v_output = cv.take(px * 4);
+    ws.partials = cv.take(bg_image_loss_num_partials(channels, h, w));
+    ws.v_combined = cv.take((uint64_t)n * BG_VCOMBINED_STRIDE);
+    ws.v_t = cv.take((uint64_t)n * 10);
+    ws.v_sh = cv.take((uint64_t)n * k * 3);
+    ws.v_o = cv.take(n);
+    ws.v_r = cv.take(n);
+    ws.visible = cv.take(n);
+    ws.max_radius = cv.take(n);
+    ws.bytes = cv.off;
     return ws;
 }
 
-// the depth step's extra scratch, behind the largest plain-step workspace
+// the depth term's scratch, from byte `off` on: behind the largest workspace of the same step without the term.  The
+// multi-view step reuses it view after view.
 struct DepthWs {
     float *depth, *v_depth, *v_z, *partials;
     uint64_t bytes;
 };
-DepthWs carve_depth_ws(void *base, uint32_t n, uint32_t k, uint32_t w, uint32_t h) {
-    uint64_t off = carve_train_ws(nullptr, n, k, w, h, 4).bytes;
-    auto take = [&](uint64_t floats) {
-        float *p = base ? reinterpret_cast<float *>(static_cast<char *>(base) + off) : nullptr;
-        off += (floats * 4 + 255) / 256 * 256;
-        return p;
-    };
+DepthWs carve_depth_ws(void *base, uint64_t off, uint32_t n, uint32_t w, uint32_t h) {
+    Carver cv{base, off};
     DepthWs ws;
     const uint64_t px = (uint64_t)w * h;
-    ws.depth = take(px);
-    ws.v_depth = take(px);
-    ws.v_z = take(std::max(n, 1u));
-    ws.partials = take(depth_loss_num_partials(h, w));
-    ws.bytes = off;
+    ws.depth = cv.take(px);
+    ws.v_depth = cv.take(px);
+    ws.v_z = cv.take(std::max(n, 1u));
+    ws.partials = cv.take(depth_loss_num_partials(h, w));
+    ws.bytes = cv.off;
     return ws;
 }
 
-// argument checks shared by bg_train_step and bg_train_step_depth
-int32_t check_train_args(const BgTrainStepArgs *a, const char *who) {
+// argument checks shared by the single-view and the multi-view steps (BgTrainStepArgs / BgTrainViewsArgs)
+template <class A>
+int32_t check_train_args(const A *a, const char *who) {
     if (!a->transforms || !a->sh || !a->raw_opac || !a->m_t || !a->v_t || !a->m_sh || !a->v_sh || !a->m_o || !a->v_o ||
         !a->refine_norm || !a->vis_weight || !a->max_screen || !a->gt_packed || !a->workspace || !a->loss_out)
         return BG_ERR_NULL;
@@ -807,20 +809,41 @@ int32_t check_train_args(const BgTrainStepArgs *a, const char *who) {
     return BG_OK;
 }
 
-// optimiser, refine statistics, mean noise (train.rs:280-416): one pass over the Gaussians
-int32_t run_train_update(BgContext *c, void *stream, const BgTrainStepArgs *a, const TrainWs &ws) {
-    BgTrainUpdateArgs up;
-    memset(&up, 0, sizeof(up));
-    up.n = a->n; up.k = a->k;
-    up.transforms = a->transforms; up.sh = a->sh; up.raw_opac = a->raw_opac;
-    up.m_t = a->m_t; up.v_t = a->v_t; up.m_sh = a->m_sh; up.v_sh = a->v_sh; up.m_o = a->m_o; up.v_o = a->v_o;
-    up.refine_norm = a->refine_norm; up.vis_weight = a->vis_weight; up.max_screen = a->max_screen;
-    up.v_transforms = ws.v_t; up.v_sh_grad = ws.v_sh; up.v_raw_opac = ws.v_o;
-    up.v_refine = ws.v_r; up.visible = ws.visible; up.max_radius = ws.max_radius;
-    up.lr_mean = a->lr_mean; up.lr_rotation = a->lr_rotation; up.lr_scale = a->lr_scale; up.lr_coeffs_dc = a->lr_coeffs_dc;
-    up.lr_coeffs_sh_scale = a->lr_coeffs_sh_scale; up.lr_opac = a->lr_opac;
-    up.noise_scale = a->noise_scale; up.median_scale = a->median_scale; up.seed = a->seed; up.step = a->step;
-    return bg_train_update(c, stream, &up);
+// Whether a view runs the depth term of DESIGN.md section 4.7.  After check_depth, a weight that is not 0 is > 0.
+bool depth_term(const BgDepthSupervision &d) { return d.weight > 0.0f && d.valid_count > 0; }
+
+int32_t check_depth(const BgDepthSupervision &d, const char *who) {
+    if (!d.depth_loss_out) return BG_ERR_NULL;
+    if (!(d.weight >= 0.0f) || !std::isfinite(d.weight)) {
+        char m[160];
+        snprintf(m, sizeof(m), "%s: weight must be finite and >= 0", who);
+        set_err(m, cudaSuccess);
+        return BG_ERR_INVALID;
+    }
+    if (depth_term(d) && !d.target) return BG_ERR_NULL;
+    return BG_OK;
+}
+
+// The loss of one rendered view into *loss (train.rs:220-260): the mean over [h,w,3] (+ alpha mean * weight), value and
+// gradient (into ws.v_output) from the fused kernel.  With d, also the depth term: v_depth, v_output[...,3] += dL/da,
+// L_d -> d->depth_loss_out and added to *loss.
+template <class A, class W>
+int32_t view_loss(BgContext *c, void *stream, const A *a, const uint32_t *gt, const W &ws, float *loss,
+                  const BgDepthSupervision *d, const DepthWs &dws) {
+    cudaStream_t s = (cudaStream_t)stream;
+    const uint32_t w = a->w, h = a->h;
+    const float npx = (float)w * (float)h;
+    float chain[4] = {1.0f / (3.0f * npx), 1.0f / (3.0f * npx), 1.0f / (3.0f * npx), a->channels == 4 ? a->alpha_weight / npx : 0.0f};
+    int32_t r = bg_image_loss_fused(c, stream, ws.out_img, gt, a->channels, h, w, 1, (int64_t)w * 4, 4, a->l1_weight, a->ssim_weight,
+                                    a->has_composite_bg ? a->composite_bg : nullptr, a->mask, chain, ws.v_output, ws.partials);
+    if (r != BG_OK) return r;
+    BG_CUDA(launch_loss_reduce(s, ws.partials, a->channels, bg_image_loss_num_partials(a->channels, h, w) / a->channels, chain, loss));
+    if (!d) return BG_OK;
+    const float dchain = d->weight / (float)d->valid_count;
+    r = bg_depth_loss_fused(c, stream, ws.out_img, dws.depth, d->target, h, w, dchain, ws.v_output, dws.v_depth, dws.partials);
+    if (r != BG_OK) return r;
+    BG_CUDA(launch_depth_loss_reduce(s, dws.partials, depth_loss_num_partials(h, w), dchain, d->depth_loss_out, loss));
+    return BG_OK;
 }
 }  // namespace
 
@@ -828,87 +851,66 @@ extern "C" uint64_t bg_train_step_workspace_bytes(uint32_t n, uint32_t k, uint32
     return carve_train_ws(nullptr, n, k, w, h, 4).bytes;
 }
 
-extern "C" int32_t bg_train_step(BgContext *c, void *stream, BgTrainStepArgs *a) {
-    if (!c || !a) return BG_ERR_NULL;
-    if (int32_t r = check_train_args(a, "bg_train_step"); r != BG_OK) return r;
+extern "C" uint64_t bg_train_step_depth_workspace_bytes(uint32_t n, uint32_t k, uint32_t w, uint32_t h) {
+    return carve_depth_ws(nullptr, bg_train_step_workspace_bytes(n, k, w, h), n, w, h).bytes;
+}
+
+// The single-view step.  d == nullptr: bg_train_step.  Otherwise the step with the depth term of DESIGN.md section 4.7
+// (d validated, its term on, by bg_train_step_depth).
+static int32_t train_step(BgContext *c, void *stream, BgTrainStepArgs *a, const BgDepthSupervision *d) {
+    if (int32_t r = check_train_args(a, d ? "bg_train_step_depth" : "bg_train_step"); r != BG_OK) return r;
     const uint32_t n = a->n, k = a->k, w = a->w, h = a->h;
     const TrainWs ws = carve_train_ws(a->workspace, n, k, w, h, a->channels);
-    if (ws.bytes > a->workspace_bytes) { set_err("bg_train_step: workspace too small (bg_train_step_workspace_bytes)", cudaSuccess); return BG_ERR_CAPACITY; }
+    // the depth term's buffers; all null without the term, which selects the plain render and blend backward
+    const DepthWs dws = carve_depth_ws(d ? a->workspace : nullptr, bg_train_step_workspace_bytes(n, k, w, h), n, w, h);
+    if ((d ? dws.bytes : ws.bytes) > a->workspace_bytes) {
+        set_err(d ? "bg_train_step_depth: workspace too small (bg_train_step_depth_workspace_bytes)"
+                  : "bg_train_step: workspace too small (bg_train_step_workspace_bytes)", cudaSuccess);
+        return BG_ERR_CAPACITY;
+    }
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
     int32_t r;
     // render forward (train.rs:200-216)
-    r = bg_render_forward(c, stream, &a->cam, w, h, n, k, a->transforms, a->sh, a->raw_opac, a->mip, a->background, BG_PASS_BACKWARD,
-                          ws.out_img, ws.visible, ws.max_radius, &a->state_out);
+    r = render_forward(c, stream, &a->cam, w, h, n, k, a->transforms, a->sh, a->raw_opac, a->mip, a->background, BG_PASS_BACKWARD,
+                       ws.out_img, dws.depth, ws.visible, ws.max_radius, &a->state_out);
     if (r != BG_OK) return r;
-    // loss value + gradient (train.rs:220-260): mean over [h,w,3] (+ alpha mean * weight)
-    const float npx = (float)w * (float)h;
-    float chain[4] = {1.0f / (3.0f * npx), 1.0f / (3.0f * npx), 1.0f / (3.0f * npx), a->channels == 4 ? a->alpha_weight / npx : 0.0f};
     BG_CUDA(cudaMemsetAsync(ws.v_output, 0, (size_t)w * h * 4 * sizeof(float), s));
-    r = bg_image_loss_fused(c, stream, ws.out_img, a->gt_packed, a->channels, h, w, 1, (int64_t)w * 4, 4, a->l1_weight, a->ssim_weight,
-                            a->has_composite_bg ? a->composite_bg : nullptr, a->mask, chain, ws.v_output, ws.partials);
+    if ((r = view_loss(c, stream, a, a->gt_packed, ws, a->loss_out, d, dws)) != BG_OK) return r;
+    // backward (bwd/burn_glue.rs:121-182); the depth gradient reaches the means through v_z
+    r = rasterize_backward(c, stream, &a->state_out, ws.out_img, dws.depth, ws.v_output, dws.v_depth, a->background, 0, ws.v_combined,
+                           n, dws.v_z, d ? "bg_rasterize_backward_depth" : "bg_rasterize_backward");
     if (r != BG_OK) return r;
-    BG_CUDA(launch_loss_reduce(s, ws.partials, a->channels, bg_image_loss_num_partials(a->channels, h, w) / a->channels, chain, a->loss_out));
-    // backward (bwd/burn_glue.rs:121-182)
-    r = bg_rasterize_backward(c, stream, &a->state_out, ws.out_img, ws.v_output, a->background, 0, ws.v_combined, n);
+    r = bg_project_backward(c, stream, &a->cam, &a->state_out, a->transforms, a->sh, a->raw_opac, ws.v_combined, ws.v_t, ws.v_sh,
+                            ws.v_o, ws.v_r);
     if (r != BG_OK) return r;
-    r = bg_project_backward(c, stream, &a->cam, &a->state_out, a->transforms, a->sh, a->raw_opac, ws.v_combined, ws.v_t, ws.v_sh, ws.v_o, ws.v_r);
-    if (r != BG_OK) return r;
-    return run_train_update(c, stream, a, ws);
+    if (d) BG_CUDA(launch_depth_to_means(s, a->state_out.compact_from_global_gid, dws.v_z, a->state_out.n, a->cam, ws.v_t));
+    // optimiser, refine statistics, mean noise (train.rs:280-416): one pass over the Gaussians, as bg_train_update
+    if (n == 0) return BG_OK;
+    UpdateParams P = update_params(a);
+    P.g_t = ws.v_t; P.g_o = ws.v_o; P.g_sh = ws.v_sh;
+    P.v_refine = ws.v_r; P.max_radius = ws.max_radius; P.visible = ws.visible;
+    BG_CUDA(launch_train_update(s, sh_degree_from_k(k), P, false));
+    return BG_OK;
+}
+
+extern "C" int32_t bg_train_step(BgContext *c, void *stream, BgTrainStepArgs *a) {
+    if (!c || !a) return BG_ERR_NULL;
+    return train_step(c, stream, a, nullptr);
 }
 
 // ---- bg_train_step_depth: bg_train_step with the depth-supervision term of DESIGN.md section 4.7
-extern "C" uint64_t bg_train_step_depth_workspace_bytes(uint32_t n, uint32_t k, uint32_t w, uint32_t h) {
-    return carve_depth_ws(nullptr, n, k, w, h).bytes;
-}
-
 extern "C" int32_t bg_train_step_depth(BgContext *c, void *stream, BgTrainStepArgs *a, const BgDepthSupervision *d) {
-    if (!c || !a || !d || !d->depth_loss_out) return BG_ERR_NULL;
-    if (!(d->weight >= 0.0f) || !std::isfinite(d->weight)) {
-        set_err("bg_train_step_depth: weight must be finite and >= 0", cudaSuccess);
-        return BG_ERR_INVALID;
-    }
-    cudaStream_t s = (cudaStream_t)stream;
-    if (d->weight == 0.0f || d->valid_count == 0) {
+    if (!c || !a || !d) return BG_ERR_NULL;
+    if (int32_t r = check_depth(*d, "bg_train_step_depth"); r != BG_OK) return r;
+    if (!depth_term(*d)) {
         // no term (target may be null): the plain step, launch for launch, and a zero depth loss
-        const int32_t r = bg_train_step(c, stream, a);
+        const int32_t r = train_step(c, stream, a, nullptr);
         if (r != BG_OK) return r;
-        BG_CUDA(cudaMemsetAsync(d->depth_loss_out, 0, sizeof(float), s));
+        BG_CUDA(cudaMemsetAsync(d->depth_loss_out, 0, sizeof(float), (cudaStream_t)stream));
         return BG_OK;
     }
-    if (!d->target) return BG_ERR_NULL;
-    if (int32_t r = check_train_args(a, "bg_train_step_depth"); r != BG_OK) return r;
-    const uint32_t n = a->n, k = a->k, w = a->w, h = a->h;
-    const TrainWs ws = carve_train_ws(a->workspace, n, k, w, h, a->channels);
-    const DepthWs dws = carve_depth_ws(a->workspace, n, k, w, h);
-    if (dws.bytes > a->workspace_bytes) {
-        set_err("bg_train_step_depth: workspace too small (bg_train_step_depth_workspace_bytes)", cudaSuccess);
-        return BG_ERR_CAPACITY;
-    }
-    BG_CUDA(cudaSetDevice(c->device));
-    int32_t r;
-    r = bg_render_forward_depth(c, stream, &a->cam, w, h, n, k, a->transforms, a->sh, a->raw_opac, a->mip, a->background,
-                                BG_PASS_BACKWARD, ws.out_img, dws.depth, ws.visible, ws.max_radius, &a->state_out);
-    if (r != BG_OK) return r;
-    const float npx = (float)w * (float)h;
-    float chain[4] = {1.0f / (3.0f * npx), 1.0f / (3.0f * npx), 1.0f / (3.0f * npx), a->channels == 4 ? a->alpha_weight / npx : 0.0f};
-    BG_CUDA(cudaMemsetAsync(ws.v_output, 0, (size_t)w * h * 4 * sizeof(float), s));
-    r = bg_image_loss_fused(c, stream, ws.out_img, a->gt_packed, a->channels, h, w, 1, (int64_t)w * 4, 4, a->l1_weight, a->ssim_weight,
-                            a->has_composite_bg ? a->composite_bg : nullptr, a->mask, chain, ws.v_output, ws.partials);
-    if (r != BG_OK) return r;
-    BG_CUDA(launch_loss_reduce(s, ws.partials, a->channels, bg_image_loss_num_partials(a->channels, h, w) / a->channels, chain, a->loss_out));
-    // depth term: v_depth, v_output[...,3] += dL/da, L_d -> depth_loss_out and added to loss_out
-    const float dchain = d->weight / (float)d->valid_count;
-    r = bg_depth_loss_fused(c, stream, ws.out_img, dws.depth, d->target, h, w, dchain, ws.v_output, dws.v_depth, dws.partials);
-    if (r != BG_OK) return r;
-    BG_CUDA(launch_depth_loss_reduce(s, dws.partials, depth_loss_num_partials(h, w), dchain, d->depth_loss_out, a->loss_out));
-    r = bg_rasterize_backward_depth(c, stream, &a->state_out, ws.out_img, dws.depth, ws.v_output, dws.v_depth, a->background, 0,
-                                    ws.v_combined, n, dws.v_z);
-    if (r != BG_OK) return r;
-    r = bg_project_backward_depth(c, stream, &a->cam, &a->state_out, a->transforms, a->sh, a->raw_opac, ws.v_combined, dws.v_z,
-                                  ws.v_t, ws.v_sh, ws.v_o, ws.v_r);
-    if (r != BG_OK) return r;
-    return run_train_update(c, stream, a, ws);
+    return train_step(c, stream, a, d);
 }
 
 // ---- view-sharded data parallelism (dp.cu): communicator, exchange, the multi-view step
@@ -1005,58 +1007,29 @@ struct ViewsWs {
     float *r_transforms, *r_opac, *v_t, *v_o, *v_color, *v_refine, *visible, *max_radius;
     uint64_t bytes;
 };
-ViewsWs carve_views_ws(void *base, uint32_t n, uint32_t k, uint32_t w, uint32_t h, uint32_t local, uint32_t world, bool fold) {
-    uint64_t off = 0;
-    auto take = [&](uint64_t floats) {
-        float *p = base ? reinterpret_cast<float *>(static_cast<char *>(base) + off) : nullptr;
-        off += (floats * 4 + 255) / 256 * 256;
-        return p;
-    };
-    (void)k;
+ViewsWs carve_views_ws(void *base, uint32_t n, uint32_t w, uint32_t h, uint32_t local, uint32_t world, bool fold) {
+    Carver cv{base};
     ViewsWs ws;
     const uint64_t px = (uint64_t)w * h;
     const DpLayout L = dp_layout(n, local, world);
-    ws.out_img = take(px * 4);
-    ws.v_output = take(px * 4);
-    ws.partials = take(bg_image_loss_num_partials(4, h, w));
-    ws.loss_terms = take(DP_MAX_VIEWS);
-    ws.v_combined = take((uint64_t)n * BG_VCOMBINED_STRIDE);
-    ws.small = take(L.small_floats);
-    ws.stat = take(L.stat_floats);
-    ws.record = take(L.rec_floats);
-    ws.recv = take(world > 1 ? L.recv_floats : 0);
-    ws.hdr = take(DP_MAX_VIEWS * 4);
-    ws.hdr_all = take(DP_MAX_VIEWS * 4);
-    ws.r_transforms = take(fold ? (uint64_t)n * 10 : 0);
-    ws.r_opac = take(fold ? n : 0);
+    ws.out_img = cv.take(px * 4);
+    ws.v_output = cv.take(px * 4);
+    ws.partials = cv.take(bg_image_loss_num_partials(4, h, w));
+    ws.loss_terms = cv.take(DP_MAX_VIEWS);
+    ws.v_combined = cv.take((uint64_t)n * BG_VCOMBINED_STRIDE);
+    ws.small = cv.take(L.small_floats);
+    ws.stat = cv.take(L.stat_floats);
+    ws.record = cv.take(L.rec_floats);
+    ws.recv = cv.take(world > 1 ? L.recv_floats : 0);
+    ws.hdr = cv.take(DP_MAX_VIEWS * 4);
+    ws.hdr_all = cv.take(DP_MAX_VIEWS * 4);
+    ws.r_transforms = cv.take(fold ? (uint64_t)n * 10 : 0);
+    ws.r_opac = cv.take(fold ? n : 0);
     // one view's gradients, as the operators write them, before they are folded into the exchange rows
-    ws.v_t = take((uint64_t)n * 10); ws.v_o = take(n); ws.v_color = take((uint64_t)n * 3); ws.v_refine = take(n);
-    ws.visible = take(n); ws.max_radius = take(n);
-    ws.bytes = off;
+    ws.v_t = cv.take((uint64_t)n * 10); ws.v_o = cv.take(n); ws.v_color = cv.take((uint64_t)n * 3); ws.v_refine = cv.take(n);
+    ws.visible = cv.take(n); ws.max_radius = cv.take(n);
+    ws.bytes = cv.off;
     return ws;
-}
-
-// the depth term's scratch of the multi-view step, behind the largest views workspace; reused view after view
-DepthWs carve_views_depth_ws(void *base, uint32_t n, uint32_t k, uint32_t w, uint32_t h, uint32_t local, uint32_t world) {
-    uint64_t off = carve_views_ws(nullptr, n, k, w, h, local, world, true).bytes;
-    auto take = [&](uint64_t floats) {
-        float *p = base ? reinterpret_cast<float *>(static_cast<char *>(base) + off) : nullptr;
-        off += (floats * 4 + 255) / 256 * 256;
-        return p;
-    };
-    DepthWs ws;
-    const uint64_t px = (uint64_t)w * h;
-    ws.depth = take(px);
-    ws.v_depth = take(px);
-    ws.v_z = take(std::max(n, 1u));
-    ws.partials = take(depth_loss_num_partials(h, w));
-    ws.bytes = off;
-    return ws;
-}
-
-// Whether view i of a multi-view depth step runs the depth term (DESIGN.md section 4.7).
-bool views_depth_term(const BgDepthSupervision *dep, uint32_t i) {
-    return dep && dep[i].weight > 0.0f && dep[i].valid_count > 0;
 }
 }  // namespace
 
@@ -1096,49 +1069,44 @@ DpTrace g_dp_trace;
 
 extern "C" uint64_t bg_train_step_views_workspace_bytes(uint32_t n, uint32_t k, uint32_t w, uint32_t h, uint32_t local,
                                                         uint32_t world) {
-    return carve_views_ws(nullptr, n, k, w, h, std::max(local, 1u), std::max(world, 1u), true).bytes;
+    (void)k;
+    return carve_views_ws(nullptr, n, w, h, std::max(local, 1u), std::max(world, 1u), true).bytes;
 }
 
 extern "C" uint64_t bg_train_step_views_depth_workspace_bytes(uint32_t n, uint32_t k, uint32_t w, uint32_t h, uint32_t local,
                                                               uint32_t world) {
-    return carve_views_depth_ws(nullptr, n, k, w, h, std::max(local, 1u), std::max(world, 1u)).bytes;
+    return carve_depth_ws(nullptr, bg_train_step_views_workspace_bytes(n, k, w, h, local, world), n, w, h).bytes;
 }
 
 // The multi-view step.  dep == nullptr: bg_train_step_views.  Otherwise dep[local_views] (validated by
 // bg_train_step_views_depth); a view whose term runs renders depth and folds its depth gradient into the exchange row, the
 // other views run exactly the plain view's launches.
 static int32_t train_step_views(BgContext *c, BgDpComm *h, void *stream, BgTrainViewsArgs *a, const BgDepthSupervision *dep) {
-    if (!c || !a) return BG_ERR_NULL;
-    if (!a->transforms || !a->sh || !a->raw_opac || !a->m_t || !a->v_t || !a->m_sh || !a->v_sh || !a->m_o || !a->v_o ||
-        !a->refine_norm || !a->vis_weight || !a->max_screen || !a->cams || !a->gt_packed || !a->workspace || !a->loss_out)
-        return BG_ERR_NULL;
+    if (!c || !a || !a->cams) return BG_ERR_NULL;
+    if (int32_t r = check_train_args(a, "bg_train_step_views"); r != BG_OK) return r;
     const uint32_t n = a->n, k = a->k, w = a->w, hh = a->h, local = a->local_views;
-    const uint32_t world = h ? (uint32_t)h->c->world : 1u, rank = h ? (uint32_t)h->c->rank : 0u;
+    const uint32_t world = h ? (uint32_t)h->c->world : 1u;
     const uint32_t views = local * world;
     if (local == 0 || views > DP_MAX_VIEWS) { set_err("bg_train_step_views: 1..16 views per step in total", cudaSuccess); return BG_ERR_INVALID; }
-    if (a->step < 1) { set_err("bg_train_step_views: step is 1-based", cudaSuccess); return BG_ERR_INVALID; }
-    if (a->channels != 3 && a->channels != 4) { set_err("bg_train_step_views: channels must be 3 or 4", cudaSuccess); return BG_ERR_INVALID; }
-    if ((uintptr_t)a->workspace % 256) { set_err("bg_train_step_views: workspace must be 256-byte aligned", cudaSuccess); return BG_ERR_INVALID; }
     const int deg = sh_degree_from_k(k);
     if (deg < 0) { set_err("Invalid nr. of sh bases", cudaSuccess); return BG_ERR_INVALID; }
     for (uint32_t i = 0; i < local; i++)
         if (!a->gt_packed[i]) return BG_ERR_NULL;
     const bool fold = a->min_scale != nullptr;
-    const ViewsWs ws = carve_views_ws(a->workspace, n, k, w, hh, local, world, fold);
+    const ViewsWs ws = carve_views_ws(a->workspace, n, w, hh, local, world, fold);
     if (ws.bytes > a->workspace_bytes) { set_err("bg_train_step_views: workspace too small (bg_train_step_views_workspace_bytes)", cudaSuccess); return BG_ERR_CAPACITY; }
     if (a->chunks > DP_MAX_CHUNKS) { set_err("bg_train_step_views: at most 16 chunks", cudaSuccess); return BG_ERR_INVALID; }
-    const DepthWs dws = carve_views_depth_ws(a->workspace, n, k, w, hh, local, world);
+    const DepthWs dws = carve_depth_ws(a->workspace, bg_train_step_views_workspace_bytes(n, k, w, hh, local, world), n, w, hh);
     if (dep && dws.bytes > a->workspace_bytes) {
         set_err("bg_train_step_views_depth: workspace too small (bg_train_step_views_depth_workspace_bytes)", cudaSuccess);
         return BG_ERR_CAPACITY;
     }
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
-    const DpLayout L = dp_layout(n, local, world);
     int32_t r;
     if (dep)
         for (uint32_t i = 0; i < local; i++)
-            if (!views_depth_term(dep, i)) BG_CUDA(cudaMemsetAsync(dep[i].depth_loss_out, 0, sizeof(float), s));
+            if (!depth_term(dep[i])) BG_CUDA(cudaMemsetAsync(dep[i].depth_loss_out, 0, sizeof(float), s));
     // the 3D-filter floor folded into what the renderer sees (bwd/burn_glue.rs:260-270)
     const float *r_t = a->transforms, *r_o = a->raw_opac;
     if (fold) {
@@ -1146,8 +1114,6 @@ static int32_t train_step_views(BgContext *c, BgDpComm *h, void *stream, BgTrain
         if (r != BG_OK) return r;
         r_t = ws.r_transforms; r_o = ws.r_opac;
     }
-    const float npx = (float)w * (float)hh;
-    float chain[4] = {1.0f / (3.0f * npx), 1.0f / (3.0f * npx), 1.0f / (3.0f * npx), a->channels == 4 ? a->alpha_weight / npx : 0.0f};
     BG_CUDA(cudaMemsetAsync(ws.v_output, 0, (size_t)w * hh * 4 * sizeof(float), s));
     DpHeader hdr;
     memset(&hdr, 0, sizeof(hdr));
@@ -1164,34 +1130,16 @@ static int32_t train_step_views(BgContext *c, BgDpComm *h, void *stream, BgTrain
     bool alpha_dirty = false;   // a depth view added to v_output[...,3], which the 3-channel image loss leaves as it is
     for (uint32_t i = 0; i < local; i++) {
         const BgCamera *cam = a->cams + i;
-        const bool term = views_depth_term(dep, i);
+        const BgDepthSupervision *di = dep && depth_term(dep[i]) ? &dep[i] : nullptr;   // the view's depth term, if it runs
+        const DepthWs vd = di ? dws : DepthWs{};   // null buffers select the plain render and blend backward
         if (alpha_dirty && a->channels == 3) BG_CUDA(cudaMemsetAsync(ws.v_output, 0, (size_t)w * hh * 4 * sizeof(float), s));
-        alpha_dirty = false;
-        if (term)
-            r = bg_render_forward_depth(c, stream, cam, w, hh, n, k, r_t, a->sh, r_o, a->mip, a->background, BG_PASS_BACKWARD, ws.out_img,
-                                        dws.depth, ws.visible, ws.max_radius, &a->state_out);
-        else
-            r = bg_render_forward(c, stream, cam, w, hh, n, k, r_t, a->sh, r_o, a->mip, a->background, BG_PASS_BACKWARD, ws.out_img,
-                                  ws.visible, ws.max_radius, &a->state_out);
+        alpha_dirty = di != nullptr;
+        r = render_forward(c, stream, cam, w, hh, n, k, r_t, a->sh, r_o, a->mip, a->background, BG_PASS_BACKWARD, ws.out_img, vd.depth,
+                           ws.visible, ws.max_radius, &a->state_out);
         if (r != BG_OK) return r;
-        r = bg_image_loss_fused(c, stream, ws.out_img, a->gt_packed[i], a->channels, hh, w, 1, (int64_t)w * 4, 4, a->l1_weight,
-                                a->ssim_weight, a->has_composite_bg ? a->composite_bg : nullptr, a->mask, chain, ws.v_output, ws.partials);
-        if (r != BG_OK) return r;
-        BG_CUDA(launch_loss_reduce(s, ws.partials, a->channels, bg_image_loss_num_partials(a->channels, hh, w) / a->channels, chain,
-                                   ws.loss_terms + i));
-        if (term) {
-            // the depth term: v_depth, v_output[...,3] += dL/da, L_d -> depth_loss_out and added to this view's loss term
-            const float dchain = dep[i].weight / (float)dep[i].valid_count;
-            r = bg_depth_loss_fused(c, stream, ws.out_img, dws.depth, dep[i].target, hh, w, dchain, ws.v_output, dws.v_depth, dws.partials);
-            if (r != BG_OK) return r;
-            BG_CUDA(launch_depth_loss_reduce(s, dws.partials, depth_loss_num_partials(hh, w), dchain, dep[i].depth_loss_out,
-                                             ws.loss_terms + i));
-            alpha_dirty = true;
-            r = bg_rasterize_backward_depth(c, stream, &a->state_out, ws.out_img, dws.depth, ws.v_output, dws.v_depth, a->background, 0,
-                                            ws.v_combined, n, dws.v_z);
-        } else {
-            r = bg_rasterize_backward(c, stream, &a->state_out, ws.out_img, ws.v_output, a->background, 0, ws.v_combined, n);
-        }
+        if ((r = view_loss(c, stream, a, a->gt_packed[i], ws, ws.loss_terms + i, di, dws)) != BG_OK) return r;
+        r = rasterize_backward(c, stream, &a->state_out, ws.out_img, vd.depth, ws.v_output, vd.v_depth, a->background, 0, ws.v_combined, n,
+                               vd.v_z, di ? "bg_rasterize_backward_depth" : "bg_rasterize_backward");
         if (r != BG_OK) return r;
         BG_CUDA(launch_pack_color(s, n, local, i, a->state_out.compact_from_global_gid, ws.v_combined, ws.record));
         if (d && i + 1 == local) {
@@ -1207,7 +1155,7 @@ static int32_t train_step_views(BgContext *c, BgDpComm *h, void *stream, BgTrain
         if (r != BG_OK) return r;
         // fold the view into the exchange rows (sum of the small gradients, MAX statistics); a depth view also folds in
         // its mean gradient v_z * R[2,:] on the way (the rounding of depth_to_means, no pass of its own)
-        if (term)
+        if (di)
             BG_CUDA(launch_pack_view_depth(s, n, local, i, i == 0, ws.v_t, ws.v_o, ws.v_refine, ws.visible, ws.max_radius,
                                            a->state_out.compact_from_global_gid, dws.v_z, *cam, ws.small, ws.stat, ws.record));
         else
@@ -1215,17 +1163,10 @@ static int32_t train_step_views(BgContext *c, BgDpComm *h, void *stream, BgTrain
                                      ws.stat, ws.record));
     }
     BG_CUDA(launch_loss_mean(s, ws.loss_terms, local, a->loss_out));
-    UpdateParams P;
-    memset(&P, 0, sizeof(P));
-    P.transforms = a->transforms; P.sh = a->sh; P.raw_opac = a->raw_opac;
-    P.m_t = a->m_t; P.v_t = a->v_t; P.m_sh = a->m_sh; P.v_sh = a->v_sh; P.m_o = a->m_o; P.v_o = a->v_o;
-    P.refine_norm = a->refine_norm; P.vis_weight = a->vis_weight; P.max_screen = a->max_screen;
+    UpdateParams P = update_params(a);
     P.small = ws.small; P.stat = ws.stat;
     P.grad_scale = 1.0f / (float)views; P.sh_grad_scale = 1.0f / (float)views;
     P.views = views; P.local = local; P.world = world;
-    P.g_begin = 0; P.count = n;
-    fill_update_consts(P, a->lr_mean, a->lr_rotation, a->lr_scale, a->lr_coeffs_dc, a->lr_coeffs_sh_scale, a->lr_opac, a->noise_scale,
-                       a->median_scale, a->seed, a->step, n);
     auto fold_back = [&]() -> int32_t {   // chain the gradients w.r.t. the folded values back to the learned ones (linear: after the sum)
         if (fold)
             BG_CUDA(launch_fold_min_scale_bwd_strided(s, n, a->transforms, a->raw_opac, a->min_scale, ws.small, ws.small + 10, DP_SMALL_ROW,
@@ -1270,13 +1211,8 @@ extern "C" int32_t bg_train_step_views_depth(BgContext *c, BgDpComm *h, void *st
     const uint32_t local = a->local_views;
     if (local == 0 || local > DP_MAX_VIEWS) { set_err("bg_train_step_views_depth: 1..16 views per step in total", cudaSuccess); return BG_ERR_INVALID; }
     for (uint32_t i = 0; i < local; i++) {
-        if (!depth[i].depth_loss_out) return BG_ERR_NULL;
-        if (!(depth[i].weight >= 0.0f) || !std::isfinite(depth[i].weight)) {
-            set_err("bg_train_step_views_depth: weight must be finite and >= 0", cudaSuccess);
-            return BG_ERR_INVALID;
-        }
-        if (views_depth_term(depth, i) && !depth[i].target) return BG_ERR_NULL;
-        if (views_depth_term(depth, i) && (uintptr_t)depth[i].target % 4) {
+        if (int32_t r = check_depth(depth[i], "bg_train_step_views_depth"); r != BG_OK) return r;
+        if (depth_term(depth[i]) && (uintptr_t)depth[i].target % 4) {
             set_err("bg_train_step_views_depth: target must be 4-byte aligned", cudaSuccess);
             return BG_ERR_INVALID;
         }
@@ -1292,20 +1228,15 @@ struct RefineWs {
     uint64_t bytes;
 };
 RefineWs carve_refine_ws(void *base, uint32_t n) {
-    uint64_t off = 0;
-    auto take = [&](uint64_t words) {
-        uint32_t *p = base ? reinterpret_cast<uint32_t *>(static_cast<char *>(base) + off) : nullptr;
-        off += (words * 4 + 255) / 256 * 256;
-        return p;
-    };
+    Carver cv{base};
+    auto take = [&](uint64_t words) { return cv.take<uint32_t>(words); };
     RefineWs w;
     w.ctl = take(64);
     w.keep = take(n); w.keep_incl = take(n); w.keys = take(n); w.vals = take(n); w.keys_s = take(n); w.vals_s = take(n);
     w.split = take(n); w.cand = take(n); w.cand_incl = take(n); w.split_incl = take(n);
-    w.refine_norm = reinterpret_cast<float *>(take(n)); w.vis_weight = reinterpret_cast<float *>(take(n));
-    w.max_screen = reinterpret_cast<float *>(take(n));
-    w.bounds_out = reinterpret_cast<float *>(take(16));
-    w.bytes = off;
+    w.refine_norm = cv.take(n); w.vis_weight = cv.take(n); w.max_screen = cv.take(n);
+    w.bounds_out = cv.take(16);
+    w.bytes = cv.off;
     return w;
 }
 }  // namespace
@@ -1424,15 +1355,10 @@ struct DecimateWs {
     uint64_t bytes;
 };
 DecimateWs carve_decimate_ws(void *base, uint32_t n) {
-    uint64_t off = 0;
-    auto take = [&](uint64_t words) {
-        uint32_t *p = base ? reinterpret_cast<uint32_t *>(static_cast<char *>(base) + off) : nullptr;
-        off += (words * 4 + 255) / 256 * 256;
-        return p;
-    };
+    Carver cv{base};
     DecimateWs w;
-    w.keys = take(n); w.vals = take(n); w.keys_s = take(n); w.vals_s = take(n);
-    w.bytes = off;
+    w.keys = cv.take<uint32_t>(n); w.vals = cv.take<uint32_t>(n); w.keys_s = cv.take<uint32_t>(n); w.vals_s = cv.take<uint32_t>(n);
+    w.bytes = cv.off;
     return w;
 }
 }  // namespace

@@ -319,13 +319,7 @@ normal_noise_kernel(uint64_t seed, uint64_t offset, uint64_t count, float *__res
     }
 }
 
-// learning-rate vectors of the train step (train.rs:328-350, config.rs:17-45) and the loss scalar
-__global__ void train_fill_lr_kernel(float *t_lr /*[10]*/, float *sh_scale /*[3k]*/, uint32_t k, float lr_mean, float lr_rotation,
-                                     float lr_scale, float sh_rest_scale) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < 10) t_lr[i] = i < 3 ? lr_mean : (i < 7 ? lr_rotation : lr_scale);
-    if (i < 3 * k) sh_scale[i] = (i < 3) ? 1.0f : sh_rest_scale;
-}
+// the loss scalar of the train step
 __global__ void __launch_bounds__(256)
 loss_reduce_kernel(const float *__restrict__ partials, uint32_t channels, uint32_t per_channel, float c0, float c1, float c2,
                    float c3, float *__restrict__ loss_out) {
@@ -360,11 +354,6 @@ cudaError_t launch_normal_noise(cudaStream_t s, uint64_t seed, uint64_t offset, 
     if (count == 0) return cudaSuccess;
     const unsigned grid = (unsigned)std::min<uint64_t>((count / 4 + 255) / 256 + 1, GRID_CAP);
     normal_noise_kernel<<<grid, 256, 0, s>>>(seed, offset, count, out);
-    return cudaGetLastError();
-}
-cudaError_t launch_train_fill_lr(cudaStream_t s, float *t_lr, float *sh_scale, uint32_t k, float lr_mean, float lr_rotation,
-                                 float lr_scale, float sh_rest_scale) {
-    train_fill_lr_kernel<<<(std::max(10u, 3 * k) + 127) / 128, 128, 0, s>>>(t_lr, sh_scale, k, lr_mean, lr_rotation, lr_scale, sh_rest_scale);
     return cudaGetLastError();
 }
 cudaError_t launch_loss_reduce(cudaStream_t s, const float *partials, uint32_t channels, uint32_t per_channel,

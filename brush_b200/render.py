@@ -171,23 +171,15 @@ def render_splats(ctx: RenderContext, camera, img_size, transforms: torch.Tensor
     max_radius = torch.empty((n,), dtype=torch.float32, device=dev)
     bg = (C.c_float * 3)(*[float(b) for b in background])
     st = _lib.BgRenderState()
-    depth = None
-    if render_depth:
-        depth = torch.empty((h, w), dtype=torch.float32, device=dev)
-        _lib.check(
-            lib.bg_render_forward_depth(ctx.handle, _stream_ptr(dev), C.byref(cam), w, h, n, k, transforms.data_ptr(),
-                                        sh_coeffs.data_ptr(), raw_opacities.data_ptr(), int(bool(mip)), bg, int(rpass),
-                                        out_img.data_ptr(), depth.data_ptr(),
-                                        visible.data_ptr() if visible is not None else None, max_radius.data_ptr(),
-                                        C.byref(st)),
-            "bg_render_forward_depth")
-    else:
-        _lib.check(
-            lib.bg_render_forward(ctx.handle, _stream_ptr(dev), C.byref(cam), w, h, n, k, transforms.data_ptr(),
-                                  sh_coeffs.data_ptr(), raw_opacities.data_ptr(), int(bool(mip)), bg, int(rpass),
-                                  out_img.data_ptr(), visible.data_ptr() if visible is not None else None,
-                                  max_radius.data_ptr(), C.byref(st)),
-            "bg_render_forward")
+    # the depth entry point takes the depth output right behind out_img
+    depth = torch.empty((h, w), dtype=torch.float32, device=dev) if render_depth else None
+    fn = "bg_render_forward_depth" if render_depth else "bg_render_forward"
+    _lib.check(
+        getattr(lib, fn)(ctx.handle, _stream_ptr(dev), C.byref(cam), w, h, n, k, transforms.data_ptr(), sh_coeffs.data_ptr(),
+                         raw_opacities.data_ptr(), int(bool(mip)), bg, int(rpass), out_img.data_ptr(),
+                         *((depth.data_ptr(),) if render_depth else ()), visible.data_ptr() if visible is not None else None,
+                         max_radius.data_ptr(), C.byref(st)),
+        fn)
     ev = None
     if not torch.cuda.is_current_stream_capturing():
         ev = torch.cuda.Event()
@@ -282,22 +274,18 @@ def project_bwd(out: RenderOutput, transforms, sh_coeffs, raw_opacities, v_combi
         v_sh = torch.empty((n, k, 3), dtype=torch.float32, device=dev)
         v_o = torch.empty((n,), dtype=torch.float32, device=dev)
         v_r = torch.empty((n,), dtype=torch.float32, device=dev)
-    if v_z is None:
-        _lib.check(
-            lib.bg_project_backward(out.ctx.handle, _stream_ptr(dev), C.byref(out.cam), C.byref(out.state),
-                                    transforms.data_ptr(), sh_coeffs.data_ptr(), raw_opacities.data_ptr(),
-                                    v_combined.data_ptr(), v_t.data_ptr(), v_sh.data_ptr(), v_o.data_ptr(), v_r.data_ptr()),
-            "bg_project_backward")
-    else:
+    if v_z is not None:
         v_z = _f32c(v_z, "v_z")
         if v_z.dim() != 1 or v_z.shape[0] < max(n, 1):
             raise ValueError("v_z must be [n] (as returned by rasterize_bwd_depth)")
-        _lib.check(
-            lib.bg_project_backward_depth(out.ctx.handle, _stream_ptr(dev), C.byref(out.cam), C.byref(out.state),
-                                          transforms.data_ptr(), sh_coeffs.data_ptr(), raw_opacities.data_ptr(),
-                                          v_combined.data_ptr(), v_z.data_ptr(), v_t.data_ptr(), v_sh.data_ptr(),
-                                          v_o.data_ptr(), v_r.data_ptr()),
-            "bg_project_backward_depth")
+    # the depth entry point takes v_z right behind v_combined
+    fn = "bg_project_backward" if v_z is None else "bg_project_backward_depth"
+    _lib.check(
+        getattr(lib, fn)(out.ctx.handle, _stream_ptr(dev), C.byref(out.cam), C.byref(out.state), transforms.data_ptr(),
+                         sh_coeffs.data_ptr(), raw_opacities.data_ptr(), v_combined.data_ptr(),
+                         *(() if v_z is None else (v_z.data_ptr(),)), v_t.data_ptr(), v_sh.data_ptr(), v_o.data_ptr(),
+                         v_r.data_ptr()),
+        fn)
     return v_t, v_sh, v_o, v_r
 
 

@@ -275,22 +275,40 @@ class SplatTrainer:
         n, k = s.num_splats(), s.sh_coeffs.shape[1]
         dev = s.transforms.device
         z = lambda *shape: torch.zeros(shape, dtype=torch.float32, device=dev)
-        scales = np.ones(k, np.float32)
-        scales[1:] = np.float32(1.0) / np.float32(self.config.lr_coeffs_sh_scale)
         self._state = dict(
             m_t=z(n, 10), v_t=z(n, 10), m_sh=z(n, k, 3), v_sh=z(n), m_o=z(n), v_o=z(n),
-            sh_lr_scale=torch.from_numpy(np.repeat(scales, 3)).to(dev),
-            t_lr=torch.zeros(10, dtype=torch.float32, device=dev),
             refine_norm=z(n), vis_weight=z(n), max_screen=z(n),
         )
 
-    def _adam(self, p, g, m, v, lr, scale, reduce_v):
-        lib = _lib.load()
-        rows = p.shape[0]
-        cols = p.numel() // max(rows, 1)
-        _lib.check(lib.bg_adam_step(self.ctx.handle, _stream_ptr(self.ctx.device), p.data_ptr(), g.data_ptr(), m.data_ptr(),
-                                    v.data_ptr(), rows, cols, scale.data_ptr() if scale is not None else None,
-                                    float(lr), 0.9, 0.999, 1e-15, self.step_count, int(reduce_v)), "bg_adam_step")
+    def _fill_state(self, a, splats: Splats) -> None:
+        """Points a train or refine argument struct at the splat parameters and the optimizer state (the structs share the
+        field names)."""
+        st = self._state
+        a.transforms, a.sh, a.raw_opac = splats.transforms.data_ptr(), splats.sh_coeffs.data_ptr(), splats.raw_opacities.data_ptr()
+        a.m_t, a.v_t, a.m_sh, a.v_sh, a.m_o, a.v_o = (st[x].data_ptr() for x in ("m_t", "v_t", "m_sh", "v_sh", "m_o", "v_o"))
+        a.refine_norm, a.vis_weight, a.max_screen = (st[x].data_ptr() for x in ("refine_norm", "vis_weight", "max_screen"))
+
+    def _fill_schedule(self, a, median_scale) -> float:
+        """Fills the learning rates, noise scale, seed and step of a train argument struct for the current step_count and
+        returns lr_mean(n) = lr_mean * decay^(n-1) * median_scale (train.rs:328-333)."""
+        cfg = self.config
+        lr_mean = cfg.lr_mean * self.lr_mean_decay ** (self.step_count - 1) * float(median_scale)
+        a.lr_mean, a.lr_rotation, a.lr_scale = float(np.float32(lr_mean)), cfg.lr_rotation, cfg.lr_scale
+        a.lr_coeffs_dc, a.lr_coeffs_sh_scale, a.lr_opac = cfg.lr_coeffs_dc, cfg.lr_coeffs_sh_scale, cfg.lr_opac
+        a.noise_scale = float(np.float32(lr_mean) * np.float32(cfg.mean_noise_weight))
+        a.median_scale, a.seed, a.step = float(median_scale), int(cfg.seed), self.step_count
+        return lr_mean
+
+    def _loss_setup(self, has_alpha: bool, masked_alpha: bool, background, h: int, w: int):
+        """The loss configuration of a view (train.rs:220-249): (l1_w, ssim_w, channels, composite, chain).  The loss is
+        the mean over [h,w,3] (+ alpha mean * weight) (train.rs:254-260), so dL/dmap is the constant chain[c] per channel."""
+        cfg = self.config
+        l1_w, ssim_w = (1.0 - cfg.ssim_weight, -cfg.ssim_weight) if self.ssim_enabled else (1.0, 0.0)
+        do_alpha_match = has_alpha and not masked_alpha and cfg.match_alpha_weight > 0.0
+        composite = background if (has_alpha and any(b != 0.0 for b in background)) else None
+        npx = float(h * w)
+        chain = [1.0 / (3.0 * npx)] * 3 + ([cfg.match_alpha_weight / npx] if do_alpha_match else [])
+        return l1_w, ssim_w, (4 if do_alpha_match else 3), composite, chain
 
     def sample_background(self):
         base = np.asarray(self.config.background_color, np.float32)
@@ -315,77 +333,44 @@ class SplatTrainer:
         return float(np.float32(self.config.depth_loss_weight) / np.float32(batch.depth_count))   # w_d / |valid|, in f32
 
     def step(self, batch: SceneBatch, splats: Splats) -> TrainStepStats:
-        if self._depth_term(batch):
-            return self._step_depth(batch, splats)
+        """One training step from the host.  A batch whose depth term runs (_depth_term) renders depth, adds the depth
+        loss (and its dL/dalpha to v_output[...,3]) and runs the depth rasterize backward and the projection backward
+        with v_z; the floor backward, the hook and the update are the same."""
         cfg = self.config
+        depth = self._depth_term(batch)
         self._ensure_state(splats)
-        st = self._state
         self.step_count += 1
         img_h, img_w = batch.img_size()
         dev = self.ctx.device
         gt_packed = batch.img_packed.to(dev, non_blocking=True)           # H2D upload (train.rs:197-198)
+        target = self._depth_target(batch) if depth else None
         background = self.sample_background()
         median_scale = self.bounds.median_size()
 
         r_transforms, r_raw_opac = splats.folded(self.ctx)   # 3D-filter floor folded in (bwd/burn_glue.rs:260-270)
         out = render_splats(self.ctx, batch.camera, (img_w, img_h), r_transforms, splats.sh_coeffs,
-                            r_raw_opac, mip=cfg.render_mip, background=background, rpass=PASS_BACKWARD)
-        # loss config (train.rs:220-249)
-        l1_w, ssim_w = (1.0 - cfg.ssim_weight, -cfg.ssim_weight) if self.ssim_enabled else (1.0, 0.0)
-        do_alpha_match = batch.has_alpha and not batch.masked_alpha and cfg.match_alpha_weight > 0.0
-        composite = background if (batch.has_alpha and any(b != 0.0 for b in background)) else None
+                            r_raw_opac, mip=cfg.render_mip, background=background, rpass=PASS_BACKWARD, render_depth=depth)
+        l1_w, ssim_w, channels, composite, chain = self._loss_setup(batch.has_alpha, batch.masked_alpha, background, img_h, img_w)
         lcfg = ImageLossConfig(l1_w, ssim_w, composite, batch.masked_alpha)
-        channels = 4 if do_alpha_match else 3
-        # loss = mean over [h,w,3] (+ alpha mean * weight) (train.rs:254-260): dL/dmap is one constant per
-        # channel, so value and gradient come from the fused kernel in one pass.
-        npx = float(img_h * img_w)
-        chain = [1.0 / (3.0 * npx)] * 3 + ([cfg.match_alpha_weight / npx] if do_alpha_match else [])
-        if self._v_output is None or self._v_output.shape != out.out_img.shape or self._v_output_ch != channels:
-            self._v_output = torch.zeros_like(out.out_img)   # channel 3 stays zero unless alpha matching
-            self._v_output_ch = channels
-        v_output, loss = image_loss_fused(self.ctx, out.out_img, gt_packed, channels, lcfg, chain, self._v_output)
-        v_combined = rasterize_bwd(out, v_output)
-        v_t, v_sh, v_o, v_r = project_bwd(out, r_transforms, splats.sh_coeffs, r_raw_opac, v_combined)
-        if splats.min_scale is not None:
-            fold_min_scale_backward(self.ctx, splats.transforms, splats.raw_opacities, splats.min_scale, v_t, v_o)
-        if self.grad_hook is not None:
-            self.grad_hook((v_t, v_sh, v_o, v_r, out.visible, out.max_radius))
-
-        lr_mean = self._apply_updates(splats, v_t, v_sh, v_o, v_r, out.visible, out.max_radius, median_scale)
-        depth_loss = torch.zeros((), dtype=torch.float32, device=dev) if batch.depth is not None else None
-        return TrainStepStats(num_visible_event=out, lr_mean=lr_mean, loss=loss, depth_loss=depth_loss)
-
-    def _step_depth(self, batch: SceneBatch, splats: Splats) -> TrainStepStats:
-        """step() with the depth term: depth render -> image loss -> depth loss (adds dL/dalpha to v_output[...,3]) ->
-        depth rasterize backward -> projection backward with v_z; the floor backward, the hook and the update as in step()."""
-        cfg = self.config
-        self._ensure_state(splats)
-        self.step_count += 1
-        img_h, img_w = batch.img_size()
-        dev = self.ctx.device
-        gt_packed = batch.img_packed.to(dev, non_blocking=True)
-        target = self._depth_target(batch)
-        background = self.sample_background()
-        median_scale = self.bounds.median_size()
-
-        r_transforms, r_raw_opac = splats.folded(self.ctx)
-        out = render_splats(self.ctx, batch.camera, (img_w, img_h), r_transforms, splats.sh_coeffs,
-                            r_raw_opac, mip=cfg.render_mip, background=background, rpass=PASS_BACKWARD, render_depth=True)
-        l1_w, ssim_w = (1.0 - cfg.ssim_weight, -cfg.ssim_weight) if self.ssim_enabled else (1.0, 0.0)
-        do_alpha_match = batch.has_alpha and not batch.masked_alpha and cfg.match_alpha_weight > 0.0
-        composite = background if (batch.has_alpha and any(b != 0.0 for b in background)) else None
-        lcfg = ImageLossConfig(l1_w, ssim_w, composite, batch.masked_alpha)
-        channels = 4 if do_alpha_match else 3
-        npx = float(img_h * img_w)
-        chain = [1.0 / (3.0 * npx)] * 3 + ([cfg.match_alpha_weight / npx] if do_alpha_match else [])
-        # a buffer of its own: the depth term writes channel 3, which the plain step's buffer keeps at zero
-        if self._v_output_depth is None or self._v_output_depth.shape != out.out_img.shape:
-            self._v_output_depth = torch.zeros_like(out.out_img)
-        elif channels == 3:
-            self._v_output_depth[..., 3].zero_()
-        v_output, loss = image_loss_fused(self.ctx, out.out_img, gt_packed, channels, lcfg, chain, self._v_output_depth)
-        v_depth, depth_loss = depth_loss_fused(self.ctx, out.out_img, out.depth, target, self._depth_chain(batch), v_output)
-        v_combined, v_z = rasterize_bwd_depth(out, v_output, v_depth)
+        if depth:
+            # a buffer of its own: the depth term writes channel 3, which the plain step's buffer keeps at zero
+            if self._v_output_depth is None or self._v_output_depth.shape != out.out_img.shape:
+                self._v_output_depth = torch.zeros_like(out.out_img)
+            elif channels == 3:
+                self._v_output_depth[..., 3].zero_()
+            v_output = self._v_output_depth
+        else:
+            if self._v_output is None or self._v_output.shape != out.out_img.shape or self._v_output_ch != channels:
+                self._v_output = torch.zeros_like(out.out_img)   # channel 3 stays zero unless alpha matching
+                self._v_output_ch = channels
+            v_output = self._v_output
+        # value and gradient of the loss from the fused kernel in one pass
+        v_output, loss = image_loss_fused(self.ctx, out.out_img, gt_packed, channels, lcfg, chain, v_output)
+        if depth:
+            v_depth, depth_loss = depth_loss_fused(self.ctx, out.out_img, out.depth, target, self._depth_chain(batch), v_output)
+            v_combined, v_z = rasterize_bwd_depth(out, v_output, v_depth)
+        else:
+            v_combined, v_z = rasterize_bwd(out, v_output), None
         v_t, v_sh, v_o, v_r = project_bwd(out, r_transforms, splats.sh_coeffs, r_raw_opac, v_combined, v_z=v_z)
         if splats.min_scale is not None:
             fold_min_scale_backward(self.ctx, splats.transforms, splats.raw_opacities, splats.min_scale, v_t, v_o)
@@ -393,8 +378,10 @@ class SplatTrainer:
             self.grad_hook((v_t, v_sh, v_o, v_r, out.visible, out.max_radius))
 
         lr_mean = self._apply_updates(splats, v_t, v_sh, v_o, v_r, out.visible, out.max_radius, median_scale)
-        return TrainStepStats(num_visible_event=out, lr_mean=lr_mean, loss=loss + depth_loss, depth_loss=depth_loss)
-
+        if depth:
+            return TrainStepStats(num_visible_event=out, lr_mean=lr_mean, loss=loss + depth_loss, depth_loss=depth_loss)
+        depth_loss = torch.zeros((), dtype=torch.float32, device=dev) if batch.depth is not None else None
+        return TrainStepStats(num_visible_event=out, lr_mean=lr_mean, loss=loss, depth_loss=depth_loss)
 
     # ------------------------------------------------------------------------------------------------
     def step_fused(self, batch: SceneBatch, splats: Splats) -> TrainStepStats:
@@ -438,31 +425,20 @@ class SplatTrainer:
 
     def _fused_args(self, batch: SceneBatch, splats: Splats, gt_packed, background, median_scale, ws, need):
         """BgTrainStepArgs of step_fused for the current step_count (loss_out left unset)."""
-        cfg, st = self.config, self._state
+        cfg = self.config
         img_h, img_w = batch.img_size()
-        n, k = splats.num_splats(), splats.sh_coeffs.shape[1]
         from .camera import build_uniforms
         a = _lib.BgTrainStepArgs()
         a.cam = _lib.camera_struct(build_uniforms(batch.camera, img_w, img_h))
-        a.w, a.h, a.n, a.k, a.mip = img_w, img_h, n, k, int(cfg.render_mip)
+        a.w, a.h, a.n, a.k, a.mip = img_w, img_h, splats.num_splats(), splats.sh_coeffs.shape[1], int(cfg.render_mip)
         for i in range(3):
-            a.background[i] = float(background[i])
-        a.transforms, a.sh, a.raw_opac = splats.transforms.data_ptr(), splats.sh_coeffs.data_ptr(), splats.raw_opacities.data_ptr()
-        a.m_t, a.v_t, a.m_sh, a.v_sh, a.m_o, a.v_o = (st[x].data_ptr() for x in ("m_t", "v_t", "m_sh", "v_sh", "m_o", "v_o"))
-        a.refine_norm, a.vis_weight, a.max_screen = (st[x].data_ptr() for x in ("refine_norm", "vis_weight", "max_screen"))
+            a.background[i] = a.composite_bg[i] = float(background[i])
+        self._fill_state(a, splats)
         a.gt_packed = gt_packed.data_ptr()
-        a.l1_weight, a.ssim_weight = (1.0 - cfg.ssim_weight, -cfg.ssim_weight) if self.ssim_enabled else (1.0, 0.0)
-        do_alpha_match = batch.has_alpha and not batch.masked_alpha and cfg.match_alpha_weight > 0.0
-        comp = batch.has_alpha and any(b != 0.0 for b in background)
-        a.has_composite_bg = int(comp)
-        for i in range(3):
-            a.composite_bg[i] = float(background[i])
-        a.mask, a.channels, a.alpha_weight = int(batch.masked_alpha), (4 if do_alpha_match else 3), float(cfg.match_alpha_weight)
-        lr_mean = cfg.lr_mean * self.lr_mean_decay ** (self.step_count - 1) * float(median_scale)
-        a.lr_mean, a.lr_rotation, a.lr_scale = float(np.float32(lr_mean)), cfg.lr_rotation, cfg.lr_scale
-        a.lr_coeffs_dc, a.lr_coeffs_sh_scale, a.lr_opac = cfg.lr_coeffs_dc, cfg.lr_coeffs_sh_scale, cfg.lr_opac
-        a.noise_scale = float(np.float32(lr_mean) * np.float32(cfg.mean_noise_weight))
-        a.median_scale, a.seed, a.step = float(median_scale), int(cfg.seed), self.step_count
+        a.l1_weight, a.ssim_weight, a.channels, composite, _ = self._loss_setup(batch.has_alpha, batch.masked_alpha, background,
+                                                                               img_h, img_w)
+        a.has_composite_bg, a.mask, a.alpha_weight = int(composite is not None), int(batch.masked_alpha), float(cfg.match_alpha_weight)
+        lr_mean = self._fill_schedule(a, median_scale)
         a.workspace, a.workspace_bytes = ws.data_ptr(), need
         return a, lr_mean
 
@@ -562,8 +538,7 @@ class SplatTrainer:
     def _views_args(self, batches, splats, ws, need, chunks):
         """BgTrainViewsArgs of step_views for the current step_count (loss_out left unset); also returns the learning rate
         and the host objects the arguments point into, which must outlive the call."""
-        cfg, st, dev = self.config, self._state, self.ctx.device
-        n, k = splats.num_splats(), splats.sh_coeffs.shape[1]
+        cfg, dev = self.config, self.ctx.device
         img_h, img_w = batches[0].img_size()
         b0 = batches[0]
         local = len(batches)
@@ -572,27 +547,19 @@ class SplatTrainer:
         median_scale = self.bounds.median_size()
         gts = [b.img_packed.to(dev, non_blocking=True) for b in batches]
         a = _lib.BgTrainViewsArgs()
-        a.w, a.h, a.n, a.k, a.mip = img_w, img_h, n, k, int(cfg.render_mip)
+        a.w, a.h, a.n, a.k, a.mip = img_w, img_h, splats.num_splats(), splats.sh_coeffs.shape[1], int(cfg.render_mip)
         for i in range(3):
-            a.background[i] = float(background[i])
-            a.composite_bg[i] = float(background[i])
+            a.background[i] = a.composite_bg[i] = float(background[i])
         a.local_views = local
         cams = (_lib.BgCamera * local)(*[_lib.camera_struct(build_uniforms(b.camera, img_w, img_h)) for b in batches])
         ptrs = (C.c_void_p * local)(*[g.data_ptr() for g in gts])
         a.cams, a.gt_packed = cams, ptrs
-        a.transforms, a.sh, a.raw_opac = splats.transforms.data_ptr(), splats.sh_coeffs.data_ptr(), splats.raw_opacities.data_ptr()
-        a.m_t, a.v_t, a.m_sh, a.v_sh, a.m_o, a.v_o = (st[x].data_ptr() for x in ("m_t", "v_t", "m_sh", "v_sh", "m_o", "v_o"))
-        a.refine_norm, a.vis_weight, a.max_screen = (st[x].data_ptr() for x in ("refine_norm", "vis_weight", "max_screen"))
+        self._fill_state(a, splats)
         a.min_scale = splats.min_scale.data_ptr() if splats.min_scale is not None else None
-        a.l1_weight, a.ssim_weight = (1.0 - cfg.ssim_weight, -cfg.ssim_weight) if self.ssim_enabled else (1.0, 0.0)
-        do_alpha_match = b0.has_alpha and not b0.masked_alpha and cfg.match_alpha_weight > 0.0
-        a.has_composite_bg = int(b0.has_alpha and any(x != 0.0 for x in background))
-        a.mask, a.channels, a.alpha_weight = int(b0.masked_alpha), (4 if do_alpha_match else 3), float(cfg.match_alpha_weight)
-        lr_mean = cfg.lr_mean * self.lr_mean_decay ** (self.step_count - 1) * float(median_scale)
-        a.lr_mean, a.lr_rotation, a.lr_scale = float(np.float32(lr_mean)), cfg.lr_rotation, cfg.lr_scale
-        a.lr_coeffs_dc, a.lr_coeffs_sh_scale, a.lr_opac = cfg.lr_coeffs_dc, cfg.lr_coeffs_sh_scale, cfg.lr_opac
-        a.noise_scale = float(np.float32(lr_mean) * np.float32(cfg.mean_noise_weight))
-        a.median_scale, a.seed, a.step, a.chunks = float(median_scale), int(cfg.seed), self.step_count, int(chunks)
+        a.l1_weight, a.ssim_weight, a.channels, composite, _ = self._loss_setup(b0.has_alpha, b0.masked_alpha, background, img_h, img_w)
+        a.has_composite_bg, a.mask, a.alpha_weight = int(composite is not None), int(b0.masked_alpha), float(cfg.match_alpha_weight)
+        lr_mean = self._fill_schedule(a, median_scale)
+        a.chunks = int(chunks)
         a.workspace, a.workspace_bytes = ws.data_ptr(), need
         return a, lr_mean, (gts, cams, ptrs)
 
@@ -600,21 +567,13 @@ class SplatTrainer:
         """Adam on the three parameter tensors, refine statistics, mean noise (train.rs:300-416): ONE pass over the
         Gaussians (bg_train_update); the noise is the counter-based draw keyed by (seed, step), identical on every
         data-parallel rank and in bg_train_step."""
-        cfg, st, dev = self.config, self._state, self.ctx.device
-        lr_mean = cfg.lr_mean * self.lr_mean_decay ** (self.step_count - 1) * float(median_scale)
-        n, k = splats.num_splats(), splats.sh_coeffs.shape[1]
         a = _lib.BgTrainUpdateArgs()
-        a.n, a.k = n, k
-        a.transforms, a.sh, a.raw_opac = splats.transforms.data_ptr(), splats.sh_coeffs.data_ptr(), splats.raw_opacities.data_ptr()
-        a.m_t, a.v_t, a.m_sh, a.v_sh, a.m_o, a.v_o = (st[x].data_ptr() for x in ("m_t", "v_t", "m_sh", "v_sh", "m_o", "v_o"))
-        a.refine_norm, a.vis_weight, a.max_screen = (st[x].data_ptr() for x in ("refine_norm", "vis_weight", "max_screen"))
+        a.n, a.k = splats.num_splats(), splats.sh_coeffs.shape[1]
+        self._fill_state(a, splats)
         a.v_transforms, a.v_sh_grad, a.v_raw_opac = v_t.data_ptr(), v_sh.data_ptr(), v_o.data_ptr()
         a.v_refine, a.visible, a.max_radius = v_r.data_ptr(), visible.data_ptr(), max_radius.data_ptr()
-        a.lr_mean, a.lr_rotation, a.lr_scale = float(np.float32(lr_mean)), cfg.lr_rotation, cfg.lr_scale
-        a.lr_coeffs_dc, a.lr_coeffs_sh_scale, a.lr_opac = cfg.lr_coeffs_dc, cfg.lr_coeffs_sh_scale, cfg.lr_opac
-        a.noise_scale = float(np.float32(lr_mean) * np.float32(cfg.mean_noise_weight))
-        a.median_scale, a.seed, a.step = float(median_scale), int(cfg.seed), self.step_count
-        _lib.check(_lib.load().bg_train_update(self.ctx.handle, _stream_ptr(dev), C.byref(a)), "bg_train_update")
+        lr_mean = self._fill_schedule(a, median_scale)
+        _lib.check(_lib.load().bg_train_update(self.ctx.handle, _stream_ptr(self.ctx.device), C.byref(a)), "bg_train_update")
         return lr_mean
 
     # ------------------------------------------------------------------------------------------------
@@ -641,9 +600,7 @@ class SplatTrainer:
         ws = torch.empty(need, dtype=torch.uint8, device=dev)
         a = _lib.BgRefineArgs()
         a.n, a.k, a.capacity = n0, k, cap
-        a.transforms, a.sh, a.raw_opac = splats.transforms.data_ptr(), splats.sh_coeffs.data_ptr(), splats.raw_opacities.data_ptr()
-        a.m_t, a.v_t, a.m_sh, a.v_sh, a.m_o, a.v_o = (st[x].data_ptr() for x in ("m_t", "v_t", "m_sh", "v_sh", "m_o", "v_o"))
-        a.refine_norm, a.vis_weight, a.max_screen = (st[x].data_ptr() for x in ("refine_norm", "vis_weight", "max_screen"))
+        self._fill_state(a, splats)
         a.transforms_out, a.sh_out, a.raw_opac_out = out["transforms"].data_ptr(), out["sh"].data_ptr(), out["raw_opac"].data_ptr()
         a.m_t_out, a.v_t_out, a.m_sh_out, a.v_sh_out, a.m_o_out, a.v_o_out = (out[x].data_ptr() for x in ("m_t", "v_t", "m_sh", "v_sh", "m_o", "v_o"))
         for i in range(3):

@@ -580,15 +580,21 @@ class SplatTrainer {
         step_ += 1;
         if (ws_.size() < need) ws_ = DeviceBuffer<unsigned char>(need);
         BgTrainStepArgs a;
-        std::memset(&a, 0, sizeof(a));
+        fill_common(a, w, h, transforms, sh_coeffs, raw_opacities, has_alpha, masked_alpha, ws_.data(), need);
         a.cam = make_uniforms(camera, w, h);
+        a.gt_packed = gt_packed;
+        return a;
+    }
+    // The fields BgTrainStepArgs and BgTrainViewsArgs share: sizes, mip, background, the trainable state, the loss setup,
+    // the schedule of step step_, the workspace and loss_out; every other field is zeroed.
+    template <class A>
+    void fill_common(A &a, uint32_t w, uint32_t h, float *transforms, float *sh_coeffs, float *raw_opacities, bool has_alpha,
+                     bool masked_alpha, void *ws, uint64_t need) {
+        std::memset(&a, 0, sizeof(a));
         a.w = w; a.h = h; a.n = n_; a.k = k_;
         a.mip = cfg_.render_mip;
         for (int i = 0; i < 3; i++) { a.background[i] = cfg_.background[i]; a.composite_bg[i] = cfg_.background[i]; }
-        a.transforms = transforms; a.sh = sh_coeffs; a.raw_opac = raw_opacities;
-        a.m_t = m_t_.data(); a.v_t = v_t_.data(); a.m_sh = m_sh_.data(); a.v_sh = v_sh_.data(); a.m_o = m_o_.data(); a.v_o = v_o_.data();
-        a.refine_norm = refine_norm_.data(); a.vis_weight = vis_weight_.data(); a.max_screen = max_screen_.data();
-        a.gt_packed = gt_packed;
+        fill_state(a, transforms, sh_coeffs, raw_opacities);
         const bool ssim = cfg_.ssim_weight > 0.0f;
         a.l1_weight = ssim ? 1.0f - cfg_.ssim_weight : 1.0f;
         a.ssim_weight = ssim ? -cfg_.ssim_weight : 0.0f;
@@ -605,9 +611,15 @@ class SplatTrainer {
         a.median_scale = median_scale_;
         a.seed = cfg_.seed;
         a.step = step_;
-        a.workspace = ws_.data(); a.workspace_bytes = need;
+        a.workspace = ws; a.workspace_bytes = need;
         a.loss_out = loss_.data();
-        return a;
+    }
+    // the splat parameters and the optimizer state (BgTrainStepArgs, BgTrainViewsArgs, BgRefineArgs)
+    template <class A>
+    void fill_state(A &a, float *transforms, float *sh_coeffs, float *raw_opacities) {
+        a.transforms = transforms; a.sh = sh_coeffs; a.raw_opac = raw_opacities;
+        a.m_t = m_t_.data(); a.v_t = v_t_.data(); a.m_sh = m_sh_.data(); a.v_sh = v_sh_.data(); a.m_o = m_o_.data(); a.v_o = v_o_.data();
+        a.refine_norm = refine_norm_.data(); a.vis_weight = vis_weight_.data(); a.max_screen = max_screen_.data();
     }
 
    public:
@@ -668,36 +680,12 @@ class SplatTrainer {
         cams.resize(local);
         for (uint32_t i = 0; i < local; i++) cams[i] = make_uniforms(cameras[i], w, h);
         BgTrainViewsArgs a;
-        std::memset(&a, 0, sizeof(a));
-        a.w = w; a.h = h; a.n = n_; a.k = k_;
-        a.mip = cfg_.render_mip;
-        for (int i = 0; i < 3; i++) { a.background[i] = cfg_.background[i]; a.composite_bg[i] = cfg_.background[i]; }
+        fill_common(a, w, h, splats.transforms.data(), splats.sh_coeffs.data(), splats.raw_opacities.data(), has_alpha, masked_alpha,
+                    views_ws_.data(), need);
         a.local_views = local;
         a.cams = cams.data();
         a.gt_packed = gt_packed.data();
-        a.transforms = splats.transforms.data(); a.sh = splats.sh_coeffs.data(); a.raw_opac = splats.raw_opacities.data();
-        a.m_t = m_t_.data(); a.v_t = v_t_.data(); a.m_sh = m_sh_.data(); a.v_sh = v_sh_.data(); a.m_o = m_o_.data(); a.v_o = v_o_.data();
-        a.refine_norm = refine_norm_.data(); a.vis_weight = vis_weight_.data(); a.max_screen = max_screen_.data();
         a.min_scale = min_scale;
-        const bool ssim = cfg_.ssim_weight > 0.0f;
-        a.l1_weight = ssim ? 1.0f - cfg_.ssim_weight : 1.0f;
-        a.ssim_weight = ssim ? -cfg_.ssim_weight : 0.0f;
-        const bool bg_nonzero = cfg_.background[0] != 0.0f || cfg_.background[1] != 0.0f || cfg_.background[2] != 0.0f;
-        a.has_composite_bg = has_alpha && bg_nonzero;
-        a.mask = masked_alpha;
-        a.channels = (has_alpha && !masked_alpha && cfg_.match_alpha_weight > 0.0f) ? 4 : 3;
-        a.alpha_weight = cfg_.match_alpha_weight;
-        const double lr_mean = cfg_.lr_mean * std::pow(decay_, (double)(step_ - 1)) * (double)median_scale_;   // train.rs:328-333
-        a.lr_mean = (float)lr_mean;
-        a.lr_rotation = cfg_.lr_rotation; a.lr_scale = cfg_.lr_scale;
-        a.lr_coeffs_dc = cfg_.lr_coeffs_dc; a.lr_coeffs_sh_scale = cfg_.lr_coeffs_sh_scale; a.lr_opac = cfg_.lr_opac;
-        a.noise_scale = (float)lr_mean * cfg_.mean_noise_weight;
-        a.median_scale = median_scale_;
-        a.seed = cfg_.seed;
-        a.step = step_;
-        a.chunks = 0;
-        a.workspace = views_ws_.data(); a.workspace_bytes = need;
-        a.loss_out = loss_.data();
         return a;
     }
 
@@ -722,9 +710,7 @@ class SplatTrainer {
         BgRefineArgs a;
         std::memset(&a, 0, sizeof(a));
         a.n = n0; a.k = k_; a.capacity = cap;
-        a.transforms = splats.transforms.data(); a.sh = splats.sh_coeffs.data(); a.raw_opac = splats.raw_opacities.data();
-        a.m_t = m_t_.data(); a.v_t = v_t_.data(); a.m_sh = m_sh_.data(); a.v_sh = v_sh_.data(); a.m_o = m_o_.data(); a.v_o = v_o_.data();
-        a.refine_norm = refine_norm_.data(); a.vis_weight = vis_weight_.data(); a.max_screen = max_screen_.data();
+        fill_state(a, splats.transforms.data(), splats.sh_coeffs.data(), splats.raw_opacities.data());
         a.transforms_out = t_out.data(); a.sh_out = sh_out.data(); a.raw_opac_out = o_out.data();
         a.m_t_out = m_t.data(); a.v_t_out = v_t.data(); a.m_sh_out = m_sh.data(); a.v_sh_out = v_sh.data(); a.m_o_out = m_o.data(); a.v_o_out = v_o.data();
         for (int i = 0; i < 3; i++) a.bounds_center[i] = bounds_.center[i];
