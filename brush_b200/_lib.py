@@ -16,7 +16,7 @@ BG_OK, BG_ERR_NULL, BG_ERR_INVALID, BG_ERR_CUDA, BG_ERR_CAPACITY, BG_ERR_UNSUPPO
 PASS_FORWARD, PASS_BACKWARD, PASS_BACKWARD_SMOOTH = 0, 1, 2
 PROJECTED_STRIDE = 16
 VCOMBINED_STRIDE = 10
-ABI_VERSION = 8
+ABI_VERSION = 9
 
 _STATUS_NAMES = {1: "BG_ERR_NULL", 2: "BG_ERR_INVALID", 3: "BG_ERR_CUDA", 4: "BG_ERR_CAPACITY", 5: "BG_ERR_UNSUPPORTED"}
 
@@ -149,6 +149,20 @@ class BgDecimateArgs(C.Structure):
     ]
 
 
+class BgCompressArgs(C.Structure):
+    _fields_ = [
+        ("n", C.c_uint32), ("k", C.c_uint32),
+        ("transforms", C.c_void_p), ("sh", C.c_void_p), ("raw_opac", C.c_void_p),
+        ("chunks_out", C.c_void_p),
+        ("packed_out", C.c_void_p),
+        ("sh_out", C.c_void_p),
+        ("order_out", C.c_void_p),
+        ("count_out", C.c_void_p),
+        ("workspace", C.c_void_p),
+        ("workspace_bytes", C.c_uint64),
+    ]
+
+
 class BgTrainViewsArgs(C.Structure):
     _fields_ = [
         ("w", C.c_uint32), ("h", C.c_uint32), ("n", C.c_uint32), ("k", C.c_uint32),
@@ -238,6 +252,8 @@ SIGNATURES = {
     "bg_pup_log_det": (_I32, [_P, _P, _U32, _P, _P]),
     "bg_decimate_workspace_bytes": (_U64, [_U32]),
     "bg_decimate_to_count": (_I32, [_P, _P, C.POINTER(BgDecimateArgs)]),
+    "bg_compress_workspace_bytes": (_U64, [_U32]),
+    "bg_compress_splats": (_I32, [_P, _P, C.POINTER(BgCompressArgs)]),
 }
 
 _lib = None

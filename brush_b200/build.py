@@ -35,6 +35,7 @@ SOURCES = {
     "refine.cu": ["-fmad=false"],
     "lod.cu": ["-fmad=false"],
     "depth_loss.cu": ["-fmad=false"],
+    "compress.cu": ["-fmad=false"],
 }
 
 

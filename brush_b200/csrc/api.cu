@@ -76,6 +76,12 @@ cudaError_t launch_pup_log_det(cudaStream_t, uint32_t, const float *, float *);
 cudaError_t launch_decimate_keys(cudaStream_t, uint32_t, const float *, uint32_t *, uint32_t *);
 cudaError_t launch_decimate_gather(cudaStream_t, uint32_t, uint32_t, const uint32_t *, const float *, const float *,
                                    const float *, const float *, float *, float *, float *, float *);
+// compress.cu
+cudaError_t launch_compress_valid_bounds(cudaStream_t, uint32_t, uint32_t, const float *, const float *, const float *,
+                                         uint32_t *, uint32_t *);
+cudaError_t launch_compress_keys(cudaStream_t, uint32_t, const float *, const uint32_t *, uint32_t *, uint32_t *);
+cudaError_t launch_compress_chunks(cudaStream_t, uint32_t, uint32_t, const float *, const float *, const float *,
+                                   const uint32_t *, const uint32_t *, float *, uint32_t *, uint8_t *, uint32_t *, uint32_t *);
 // depth_loss.cu
 uint32_t depth_loss_num_partials(uint32_t, uint32_t);
 cudaError_t launch_depth_loss_fused(cudaStream_t, const float *, const float *, const float *, uint32_t, uint32_t, float, float *,
@@ -1389,5 +1395,57 @@ extern "C" int32_t bg_decimate_to_count(BgContext *c, void *stream, const BgDeci
     BG_CUDA(launch_decimate_gather(s, target, a->k * 3, w.vals_s, a->transforms, a->sh, a->raw_opac, a->min_scale,
                                    a->transforms_out, a->sh_out, a->raw_opac_out, a->min_scale_out));
     if (a->kept_ids_out) BG_CUDA(cudaMemcpyAsync(a->kept_ids_out, w.vals_s, (size_t)target * 4, cudaMemcpyDeviceToDevice, s));
+    return BG_OK;
+}
+
+// ---- Compressed PLY encoding (compress.cu, DESIGN.md section 4.8)
+namespace {
+struct CompressWs {
+    uint32_t *bounds, *keys, *vals, *keys_s, *vals_s;
+    uint64_t bytes;
+};
+CompressWs carve_compress_ws(void *base, uint32_t n) {
+    Carver cv{base};
+    CompressWs w;
+    w.bounds = cv.take<uint32_t>(8);
+    w.keys = cv.take<uint32_t>(n); w.vals = cv.take<uint32_t>(n); w.keys_s = cv.take<uint32_t>(n); w.vals_s = cv.take<uint32_t>(n);
+    w.bytes = cv.off;
+    return w;
+}
+}  // namespace
+
+extern "C" uint64_t bg_compress_workspace_bytes(uint32_t n) { return carve_compress_ws(nullptr, std::max(n, 1u)).bytes; }
+
+extern "C" int32_t bg_compress_splats(BgContext *c, void *stream, const BgCompressArgs *a) {
+    if (!c || !a) return BG_ERR_NULL;
+    const uint32_t n = a->n, k = a->k;
+    if (!a->count_out) return BG_ERR_NULL;
+    if (sh_degree_from_k(k) < 0) { set_err("Invalid nr. of sh bases", cudaSuccess); return BG_ERR_INVALID; }
+    if ((uintptr_t)a->count_out % 4) { set_err("bg_compress_splats: count_out must be 4-byte aligned", cudaSuccess); return BG_ERR_INVALID; }
+    cudaStream_t s = (cudaStream_t)stream;
+    if (n == 0) {
+        BG_CUDA(cudaSetDevice(c->device));
+        BG_CUDA(cudaMemsetAsync(a->count_out, 0, 4, s));
+        return BG_OK;
+    }
+    if (!a->transforms || !a->sh || !a->raw_opac || !a->chunks_out || !a->packed_out || !a->workspace || (k > 1 && !a->sh_out))
+        return BG_ERR_NULL;
+    if (k == 1 && a->sh_out) { set_err("bg_compress_splats: sh_out must be NULL when k == 1", cudaSuccess); return BG_ERR_INVALID; }
+    if (((uintptr_t)a->transforms | (uintptr_t)a->packed_out) % 16 ||
+        ((uintptr_t)a->sh | (uintptr_t)a->raw_opac | (uintptr_t)a->chunks_out | (uintptr_t)a->order_out) % 4) {
+        set_err("bg_compress_splats: transforms and packed_out must be 16-byte aligned, the other arrays 4-byte", cudaSuccess);
+        return BG_ERR_INVALID;
+    }
+    if ((uintptr_t)a->workspace % 256) { set_err("bg_compress_splats: workspace must be 256-byte aligned", cudaSuccess); return BG_ERR_INVALID; }
+    const CompressWs w = carve_compress_ws(a->workspace, n);
+    if (w.bytes > a->workspace_bytes) { set_err("bg_compress_splats: workspace too small (bg_compress_workspace_bytes)", cudaSuccess); return BG_ERR_CAPACITY; }
+    if (n > std::max(c->max_n, c->max_isect)) { set_err("bg_compress_splats: n exceeds the context's sort capacity", cudaSuccess); return BG_ERR_CAPACITY; }
+    BG_CUDA(cudaSetDevice(c->device));
+    BG_CUDA(launch_compress_valid_bounds(s, n, k * 3, a->transforms, a->sh, a->raw_opac, w.keys, w.bounds));
+    BG_CUDA(launch_compress_keys(s, n, a->transforms, w.bounds, w.keys, w.vals));
+    int32_t r = bg_radix_argsort_u32(c, stream, w.keys, w.vals, n, nullptr, 31, w.keys_s, w.vals_s);
+    if (r != BG_OK) return r;
+    BG_CUDA(launch_compress_chunks(s, n, k, a->transforms, a->sh, a->raw_opac, w.bounds, w.vals_s, a->chunks_out, a->packed_out,
+                                   a->sh_out, a->order_out, a->count_out));
     return BG_OK;
 }

@@ -25,6 +25,7 @@ class ProcessConfig:                     # brush-process/src/config.rs (the fiel
     start_iter: int = 0
     seed: int = 42
     eval_save_to_disk: bool = False     # the rendered eval images go to <export_path>/eval_<iter>/<image name>.png
+    export_compressed: bool = False     # exports (every LOD level included) use the SuperSplat compressed layout
 
 
 def should_refine(it: int, refine_every: int, total_iters: int) -> bool:
@@ -104,6 +105,7 @@ def train_loop(ctx, splats, train_views: Sequence, eval_views: Sequence, config,
     dataset.SceneView lists."""
     import torch
     from . import ply
+    from .compress import splat_to_compressed_ply
     from .dataset import SceneLoader
     from .eval import eval_stats
     from .lod import compute_pup_scores, decimate_to_count, lod_target_count
@@ -142,8 +144,11 @@ def train_loop(ctx, splats, train_views: Sequence, eval_views: Sequence, config,
 
     def export(name: str):
         t_fold, o_fold = splats.folded(ctx)                # export.rs:183: the floor is folded into a COPY, never stored
-        data = ply.splat_to_ply(t_fold.cpu().numpy(), splats.sh_coeffs.cpu().numpy(), o_fold.cpu().numpy(),
-                                render_mip=config.render_mip)
+        if process.export_compressed:
+            data = splat_to_compressed_ply(ctx, t_fold, splats.sh_coeffs, o_fold, render_mip=config.render_mip)
+        else:
+            data = ply.splat_to_ply(t_fold.cpu().numpy(), splats.sh_coeffs.cpu().numpy(), o_fold.cpu().numpy(),
+                                    render_mip=config.render_mip)
         os.makedirs(process.export_path, exist_ok=True)
         with open(os.path.join(process.export_path, name), "wb") as f:
             f.write(data)

@@ -9,6 +9,8 @@
   _load_compressed_ply <- import.rs:408-600, ply_gaussian.rs:23-34,102-122, quant.rs:1-71: the SuperSplat compressed
                        variant (per-256-splat quantisation ranges in a leading `chunk` element, 11/10/11-bit positions and
                        scales, smallest-three quaternions, 8-bit colour + opacity, optional 8-bit higher SH bands)
+  compressed_ply_bytes <- no reference writer: the same layout from an encoding made on the device
+                       (compress.splat_to_compressed_ply, DESIGN.md section 4.8)
 
 Storage format, not part of the per-step hot path: numpy on the host, one pass.
 """
@@ -63,6 +65,14 @@ def splat_to_ply(transforms: np.ndarray, sh_coeffs: np.ndarray, raw_opacities: n
     out[:, 11:14] = chan_major[:, :, 0]
     if rest:
         out[:, 14:] = chan_major[:, :, 1:].reshape(n, 3 * rest)
+    comments = export_comments(degree, up_axis, render_mip)
+    head = ["ply", "format binary_little_endian 1.0"] + [f"comment {c}" for c in comments] + [f"element vertex {n}"]
+    head += [f"property float {nm}" for nm in names] + ["end_header"]
+    return ("\n".join(head) + "\n").encode("ascii") + out.astype("<f4").tobytes()
+
+
+def export_comments(degree: int, up_axis=None, render_mip: bool = False):
+    """The header comments of an exported file (export.rs:188-196)."""
     comments = ["Exported from Brush"]
     if up_axis is not None:
         comments.append("Vertical axis: {} {} {}".format(*[_fmt_f32(v) for v in up_axis]))
@@ -70,9 +80,7 @@ def splat_to_ply(transforms: np.ndarray, sh_coeffs: np.ndarray, raw_opacities: n
         comments.append("Vertical axis: y")
     comments.append(f"SH degree: {degree}")
     comments.append("SplatRenderMode: " + ("mip" if render_mip else "default"))
-    head = ["ply", "format binary_little_endian 1.0"] + [f"comment {c}" for c in comments] + [f"element vertex {n}"]
-    head += [f"property float {nm}" for nm in names] + ["end_header"]
-    return ("\n".join(head) + "\n").encode("ascii") + out.astype("<f4").tobytes()
+    return comments
 
 
 def _fmt_f32(v) -> str:
@@ -372,3 +380,25 @@ def _load_compressed_ply(data: bytes, fmt: str, comments, elements, off: int, su
                 sh[:, 1:, :] = rest[:, :3 * per].reshape(n, 3, per).transpose(0, 2, 1)                  # interleave_coeffs
     d = SplatData(means=means, rotations=rotations, log_scales=log_scales, sh_coeffs=sh, raw_opacities=opacity)
     return d, ParseMetadata(up_axis=_up_axis(comments), render_mip=_render_mode(comments), total_splats=n)
+
+
+COMPRESSED_VERTEX_FIELDS = ("packed_position", "packed_rotation", "packed_scale", "packed_color")
+
+
+def compressed_ply_bytes(chunks: np.ndarray, packed: np.ndarray, sh_bytes: Optional[np.ndarray], m: int, comments) -> bytes:
+    """The SuperSplat compressed layout that _load_compressed_ply reads, from an encoding (DESIGN.md section 4.8):
+    chunks [ceil(m/256), 18] f32 in _QUANT_META_FIELDS order, packed [m, 4] u32 (COMPRESSED_VERTEX_FIELDS),
+    sh_bytes [m, 3(K-1)] u8 channel-major or None for K == 1.  Binary little-endian."""
+    m = int(m)
+    n_chunks = (m + 255) // 256
+    chunks = np.ascontiguousarray(chunks, np.float32).reshape(-1, 18)[:n_chunks]
+    packed = np.ascontiguousarray(packed, np.uint32).reshape(-1, 4)[:m]
+    rest = 0 if sh_bytes is None else int(sh_bytes.shape[1])
+    head = ["ply", "format binary_little_endian 1.0"] + [f"comment {c}" for c in comments]
+    head += [f"element chunk {n_chunks}"] + [f"property float {nm}" for nm in _QUANT_META_FIELDS]
+    head += [f"element vertex {m}"] + [f"property uint {nm}" for nm in COMPRESSED_VERTEX_FIELDS]
+    body = chunks.astype("<f4").tobytes() + packed.astype("<u4").tobytes()
+    if rest:
+        head += [f"element sh {m}"] + [f"property uchar f_rest_{i}" for i in range(rest)]
+        body += np.ascontiguousarray(sh_bytes[:m], np.uint8).tobytes()
+    return ("\n".join(head + ["end_header"]) + "\n").encode("ascii") + body

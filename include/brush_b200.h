@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define BG_ABI_VERSION 8u
+#define BG_ABI_VERSION 9u
 
 /* f32 lanes per projected splat: a 64-byte row, four aligned 128-bit loads.  Lanes 0..8 are the reference
  * layout (kernels/helpers.rs:49-53: xy_x, xy_y, conic_x, conic_y, conic_z, color_a, color_r, color_g, color_b).
@@ -375,6 +375,29 @@ typedef struct {
 } BgDecimateArgs;
 uint64_t bg_decimate_workspace_bytes(uint32_t n);
 int32_t bg_decimate_to_count(BgContext *ctx, void *stream, const BgDecimateArgs *args);
+
+/* ---- SuperSplat compressed PLY encoding (the inverse of import.rs:408-600; DESIGN.md section 4.8 fixes every rounding).
+ * Rows with a non-finite float or a quaternion of zero squared norm are dropped; the m kept rows are ordered along a 30-bit
+ * Morton curve over the kept means' bounding box (the context's stable radix sort, ties in index order) and split into
+ * chunks of 256 rows.  Per chunk: 18 floats (min/max of x, y, z, the three log-scales and rgb = f_dc * SH_C0 + 0.5, in
+ * the importer's field order).  Per row: position and log-scale at 11/10/11 bits, the smallest-three quaternion, 8-bit rgb
+ * and opacity (1..254), and 3(k-1) bytes of higher SH bands, channel-major.  The inputs are what the float export writes
+ * (the Mip floor already folded).  Nothing is read back: count_out receives m on the device, and rows >= m of the
+ * outputs are left untouched.  n <= the context's sort capacity, else BG_ERR_CAPACITY.  transforms and packed_out
+ * 16-byte aligned, workspace 256-byte aligned, the other arrays 4-byte aligned. */
+typedef struct {
+    uint32_t n, k;
+    const float *transforms, *sh, *raw_opac;   /* [n,10] [n,k,3] [n], floor already folded */
+    float *chunks_out;                         /* [ceil(n/256), 18] */
+    uint32_t *packed_out;                      /* [n, 4]: position, rotation, scale, color */
+    uint8_t *sh_out;                           /* [n, 3(k-1)] channel-major; NULL iff k == 1 */
+    uint32_t *order_out;                       /* [n] source row of each output row, or NULL */
+    uint32_t *count_out;                       /* device scalar: m */
+    void *workspace;
+    uint64_t workspace_bytes;                  /* >= bg_compress_workspace_bytes(n) */
+} BgCompressArgs;
+uint64_t bg_compress_workspace_bytes(uint32_t n);
+int32_t bg_compress_splats(BgContext *ctx, void *stream, const BgCompressArgs *args);
 
 /* ---- View-sharded data parallelism behind the boundary (SURVEY.md section 8e; the reference is single-device).
  * A communicator is one NCCL rank bound to the context's device.  Rank 0 calls bg_dp_unique_id and ships the 128 bytes

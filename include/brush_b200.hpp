@@ -18,6 +18,8 @@
 //   Splats                      <- brush-render/src/gaussian_splats.rs:57-74 (owns the three parameter tensors)
 //   DpComm                      <- no reference counterpart (SURVEY.md 8e): one NCCL rank per context, behind the ABI
 //   pup_scores, decimate_to_count <- LOD baking, brush-train/src/lod.rs:13-142 (bg_pup_*, bg_decimate_to_count)
+//   compress_splats, compressed_ply_bytes <- SuperSplat compressed PLY export (bg_compress_splats; the reference only reads
+//                                  the layout, brush-serde/src/import.rs:408-600)
 //
 // Errors: the reference panics on shape / device violations (render.rs:50-64); here every non-zero ABI status
 // becomes a brush_b200::Error (std::runtime_error) carrying the status and bg_last_error_string().
@@ -848,6 +850,81 @@ inline void decimate_to_count(Context &ctx, cudaStream_t stream, Splats &splats,
     splats.n = target;
     if (floor) *min_scale = std::move(f_out);
     if (kept_ids) *kept_ids = std::move(ids);
+}
+
+// ---------------------------------------------------------------------------------------------- compressed PLY export
+// The SuperSplat compressed encoding of device splats (bg_compress_splats, DESIGN.md section 4.8), copied to the host:
+// the kept rows only, in Morton order.
+struct CompressedSplats {
+    uint32_t count = 0, k = 1;
+    std::vector<float> chunks;       // [ceil(count/256), 18]
+    std::vector<uint32_t> packed;    // [count, 4]: position, rotation, scale, color
+    std::vector<uint8_t> sh;         // [count, 3(k-1)] channel-major
+    std::vector<uint32_t> order;     // [count] source row of each output row
+};
+
+// transforms [n,10], sh [n,k,3], raw_opac [n]: device arrays, the Mip floor already folded.  One synchronise to read the
+// kept count, then copies of the encoded rows.
+inline CompressedSplats compress_splats(Context &ctx, cudaStream_t stream, const float *transforms, const float *sh,
+                                        const float *raw_opac, uint32_t n, uint32_t k) {
+    const uint32_t rest = 3 * (k - 1), n_chunks = (n + 255) / 256;
+    DeviceBuffer<float> chunks((size_t)n_chunks * 18);
+    DeviceBuffer<uint32_t> packed((size_t)n * 4), order(n), count(1);
+    DeviceBuffer<uint8_t> sh_out(k > 1 ? (size_t)n * rest : 0);
+    const uint64_t need = bg_compress_workspace_bytes(n);
+    DeviceBuffer<unsigned char> ws(need);
+    BgCompressArgs a;
+    std::memset(&a, 0, sizeof(a));
+    a.n = n; a.k = k;
+    a.transforms = transforms; a.sh = sh; a.raw_opac = raw_opac;
+    a.chunks_out = chunks.data(); a.packed_out = packed.data(); a.sh_out = k > 1 ? sh_out.data() : nullptr;
+    a.order_out = order.data(); a.count_out = count.data();
+    a.workspace = ws.data(); a.workspace_bytes = need;
+    check(bg_compress_splats(ctx.handle(), stream, &a), "compress_splats");
+    CompressedSplats out;
+    out.k = k;
+    count.download(&out.count, 1, stream);
+    const uint32_t m = out.count;
+    out.chunks.resize((size_t)(m + 255) / 256 * 18); out.packed.resize((size_t)m * 4); out.order.resize(m);
+    out.sh.resize((size_t)m * (k > 1 ? rest : 0));
+    if (m) {
+        chunks.download(out.chunks.data(), out.chunks.size(), stream);
+        packed.download(out.packed.data(), out.packed.size(), stream);
+        order.download(out.order.data(), m, stream);
+        if (k > 1) sh_out.download(out.sh.data(), out.sh.size(), stream);
+    }
+    return out;
+}
+
+// The comments of an exported file with the default vertical axis (export.rs:188-196).
+inline std::vector<std::string> export_comments(uint32_t k, bool render_mip = false) {
+    const int degree = (int)std::lround(std::sqrt((double)k)) - 1;
+    return {"Exported from Brush", "Vertical axis: y", "SH degree: " + std::to_string(degree),
+            std::string("SplatRenderMode: ") + (render_mip ? "mip" : "default")};
+}
+
+// The file bytes, identical to brush_b200.ply.compressed_ply_bytes (binary little-endian; this header assumes a
+// little-endian host, as the ABI does).
+inline std::string compressed_ply_bytes(const CompressedSplats &c, const std::vector<std::string> &comments) {
+    static const char *meta[18] = {"min_x", "max_x", "min_y", "max_y", "min_z", "max_z", "min_scale_x", "max_scale_x",
+                                   "min_scale_y", "max_scale_y", "min_scale_z", "max_scale_z", "min_r", "max_r", "min_g",
+                                   "max_g", "min_b", "max_b"};
+    const uint32_t m = c.count, rest = 3 * (c.k - 1), n_chunks = (m + 255) / 256;
+    std::string s = "ply\nformat binary_little_endian 1.0\n";
+    for (const std::string &cm : comments) s += "comment " + cm + "\n";
+    s += "element chunk " + std::to_string(n_chunks) + "\n";
+    for (const char *f : meta) s += std::string("property float ") + f + "\n";
+    s += "element vertex " + std::to_string(m) + "\n";
+    for (const char *f : {"packed_position", "packed_rotation", "packed_scale", "packed_color"}) s += std::string("property uint ") + f + "\n";
+    if (rest) {
+        s += "element sh " + std::to_string(m) + "\n";
+        for (uint32_t i = 0; i < rest; i++) s += "property uchar f_rest_" + std::to_string(i) + "\n";
+    }
+    s += "end_header\n";
+    s.append(reinterpret_cast<const char *>(c.chunks.data()), (size_t)n_chunks * 18 * sizeof(float));
+    s.append(reinterpret_cast<const char *>(c.packed.data()), (size_t)m * 4 * sizeof(uint32_t));
+    if (rest) s.append(reinterpret_cast<const char *>(c.sh.data()), (size_t)m * rest);
+    return s;
 }
 
 }  // namespace brush_b200
