@@ -16,7 +16,7 @@ BG_OK, BG_ERR_NULL, BG_ERR_INVALID, BG_ERR_CUDA, BG_ERR_CAPACITY, BG_ERR_UNSUPPO
 PASS_FORWARD, PASS_BACKWARD, PASS_BACKWARD_SMOOTH = 0, 1, 2
 PROJECTED_STRIDE = 16
 VCOMBINED_STRIDE = 10
-ABI_VERSION = 9
+ABI_VERSION = 10
 
 _STATUS_NAMES = {1: "BG_ERR_NULL", 2: "BG_ERR_INVALID", 3: "BG_ERR_CUDA", 4: "BG_ERR_CAPACITY", 5: "BG_ERR_UNSUPPORTED"}
 
@@ -105,6 +105,7 @@ class BgTrainUpdateArgs(C.Structure):
         ("noise_scale", C.c_float), ("median_scale", C.c_float),
         ("seed", C.c_uint64),
         ("step", C.c_int32),
+        ("min_scale", C.c_void_p),
     ]
 
 

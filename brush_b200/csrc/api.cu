@@ -723,6 +723,13 @@ static UpdateParams update_params(const A *a) {
     return P;
 }
 
+// The update pass reads the transforms rows and their moments as float2 and the SH spans as float4.
+template <class A>
+static bool update_aligned(const A *a) {
+    return (uintptr_t)a->transforms % 8 == 0 && (uintptr_t)a->m_t % 8 == 0 && (uintptr_t)a->v_t % 8 == 0 &&
+           (uintptr_t)a->sh % 16 == 0 && (uintptr_t)a->m_sh % 16 == 0;
+}
+
 extern "C" int32_t bg_train_update(BgContext *c, void *stream, const BgTrainUpdateArgs *a) {
     if (!c || !a) return BG_ERR_NULL;
     if (a->n == 0) return BG_OK;
@@ -733,10 +740,16 @@ extern "C" int32_t bg_train_update(BgContext *c, void *stream, const BgTrainUpda
     const int deg = sh_degree_from_k(a->k);
     if (deg < 0) { set_err("Invalid nr. of sh bases", cudaSuccess); return BG_ERR_INVALID; }
     if (a->step < 1) { set_err("bg_train_update: step is 1-based", cudaSuccess); return BG_ERR_INVALID; }
+    if (!update_aligned(a) || (uintptr_t)a->v_transforms % 8 || (uintptr_t)a->v_sh_grad % 16) {
+        set_err("bg_train_update: transforms, m_t, v_t and v_transforms must be 8-byte aligned, sh, m_sh and v_sh_grad "
+                "16-byte aligned (64- and 128-bit row access)", cudaSuccess);
+        return BG_ERR_INVALID;
+    }
     BG_CUDA(cudaSetDevice(c->device));
     UpdateParams P = update_params(a);
     P.g_t = a->v_transforms; P.g_o = a->v_raw_opac; P.g_sh = a->v_sh_grad;
     P.v_refine = a->v_refine; P.max_radius = a->max_radius; P.visible = a->visible;
+    P.min_scale = a->min_scale;
     BG_CUDA(launch_train_update((cudaStream_t)stream, deg, P, false));
     return BG_OK;
 }
@@ -812,6 +825,7 @@ int32_t check_train_args(const A *a, const char *who) {
     if (a->step < 1) return invalid("step is 1-based");
     if (a->channels != 3 && a->channels != 4) return invalid("channels must be 3 or 4");
     if ((uintptr_t)a->workspace % 256) return invalid("workspace must be 256-byte aligned");
+    if (!update_aligned(a)) return invalid("transforms, m_t and v_t must be 8-byte aligned, sh and m_sh 16-byte aligned");
     return BG_OK;
 }
 
@@ -1170,6 +1184,7 @@ static int32_t train_step_views(BgContext *c, BgDpComm *h, void *stream, BgTrain
     }
     BG_CUDA(launch_loss_mean(s, ws.loss_terms, local, a->loss_out));
     UpdateParams P = update_params(a);
+    P.min_scale = a->min_scale;   // the noise gate folds the floor in, as the render did
     P.small = ws.small; P.stat = ws.stat;
     P.grad_scale = 1.0f / (float)views; P.sh_grad_scale = 1.0f / (float)views;
     P.views = views; P.local = local; P.world = world;

@@ -29,6 +29,7 @@ struct UpdateParams {
     int noisy;
     float noise_scale, median_scale;
     unsigned long long seed, noise_offset;
+    const float *min_scale;          // [n] 3D-filter floor or null: the noise gate uses the folded opacity (bg_fold.cuh)
 };
 
 cudaError_t launch_train_update(cudaStream_t s, int deg, const UpdateParams &P, bool factored, int part = 0);

@@ -12,6 +12,7 @@
 #include <algorithm>
 
 #include "bg_common.cuh"
+#include "bg_fold.cuh"
 #include "bg_rng.cuh"
 
 namespace bg {
@@ -213,27 +214,6 @@ min_scale_kernel(uint32_t n, const float *__restrict__ transforms, const float *
         }
     }
     if (i < n) f_out[i] = best * sqrt_factor;
-}
-
-struct FoldTerms { float s2[3], s2f[3], coef, sig, opac; bool in_range; };
-
-__device__ __forceinline__ FoldTerms fold_terms(const float *ls, float raw, float f) {
-    FoldTerms t;
-    const float f2 = f * f;
-    float det1 = 1.f, det2 = 1.f;
-#pragma unroll
-    for (int a = 0; a < 3; a++) {
-        t.s2[a] = expf(2.0f * ls[a]);
-        t.s2f[a] = t.s2[a] + f2;
-    }
-    det1 = t.s2[0] * t.s2[1] * t.s2[2];
-    det2 = t.s2f[0] * t.s2f[1] * t.s2f[2];
-    t.coef = sqrtf(det1 / det2);
-    t.sig = 1.0f / (1.0f + expf(-raw));
-    const float o = t.sig * t.coef;
-    t.in_range = o >= 1e-6f && o <= 1.0f - 1e-6f;
-    t.opac = fminf(fmaxf(o, 1e-6f), 1.0f - 1e-6f);
-    return t;
 }
 
 // transforms_out may alias transforms (bake_min_scale, gaussian_splats.rs:245-252).

@@ -3,7 +3,9 @@
 //   AdamScaled::step on transforms [N,10] (per-column LR), SH coefficients [N,K,3] (per-band LR, second moment =
 //   row mean of g^2) and raw opacity [N]                               (adam_scaled.rs:75-165, train.rs:328-381)
 //   RefineRecord::gather_stats (MAX refine weight, SUM visible, MAX radius)            (stats.rs:40-50)
-//   the mean noise  means += clamp(N(0,1) (1-sigmoid(opac'))^150 vis lr 50, +-median)    (train.rs:389-416)
+//   the mean noise  means += clamp(N(0,1) (1-opacity')^150 [vis > 0] lr 50, +-median)    (train.rs:389-416)
+//   (opacity' = sigmoid(raw'), or with a floor clamp(sigmoid(raw') coef(log_scales', f), 1e-6, 1-1e-6); the gate is
+//   visible > 0, which for the summed counts of a multi-view step is "seen by some view")
 // The reference issues ~80 generic tensor ops for this; round 1 used five kernels (3 Adam, noise draw, stats+noise).
 // A warp owns 32 consecutive Gaussians: the short rows (transforms, opacity, statistics) one lane each, the SH rows as
 // one contiguous span read and written with coalesced 128-bit accesses; the normal
@@ -22,6 +24,7 @@
 #include <algorithm>
 
 #include "bg_common.cuh"
+#include "bg_fold.cuh"
 #include "bg_rng.cuh"
 #include "bg_sh.cuh"
 #include "bg_update.cuh"
@@ -131,9 +134,11 @@ train_update_kernel(const UpdateParams P) {
             P.vis_weight[i] = P.vis_weight[i] + vis;
             P.max_screen[i] = fmaxf(rad, P.max_screen[i]);
         }
-        // ---- mean noise on the updated means, gated by the updated opacity (train.rs:389-416)
+        // ---- mean noise on the updated means, gated by the updated opacity (train.rs:389-416).  The reference gates on
+        // Splats::opacities(), which folds the floor in when there is one (gaussian_splats.rs:215-223): then the gate is
+        // clamp(sigmoid(raw) coef, 1e-6, 1-1e-6) with coef from the updated log-scales.
         if (P.noisy) {
-            const float opac = 1.0f / (1.0f + expf(-raw));
+            const float opac = P.min_scale ? fold_terms(p + 7, raw, __ldg(P.min_scale + i)).opac : 1.0f / (1.0f + expf(-raw));
             const float wgt = fminf(fmaxf(powf(1.0f - opac, 150.0f), 0.0f), 1.0f) * (vis > 0.0f ? 1.0f : 0.0f);
             const float wm = wgt * P.noise_scale;
             if (wm != 0.0f) {

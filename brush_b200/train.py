@@ -566,10 +566,11 @@ class SplatTrainer:
     def _apply_updates(self, splats, v_t, v_sh, v_o, v_r, visible, max_radius, median_scale) -> float:
         """Adam on the three parameter tensors, refine statistics, mean noise (train.rs:300-416): ONE pass over the
         Gaussians (bg_train_update); the noise is the counter-based draw keyed by (seed, step), identical on every
-        data-parallel rank and in bg_train_step."""
+        data-parallel rank and in bg_train_step.  With a floor, the noise is gated on the folded opacity."""
         a = _lib.BgTrainUpdateArgs()
         a.n, a.k = splats.num_splats(), splats.sh_coeffs.shape[1]
         self._fill_state(a, splats)
+        a.min_scale = splats.min_scale.data_ptr() if splats.min_scale is not None else None
         a.v_transforms, a.v_sh_grad, a.v_raw_opac = v_t.data_ptr(), v_sh.data_ptr(), v_o.data_ptr()
         a.v_refine, a.visible, a.max_radius = v_r.data_ptr(), visible.data_ptr(), max_radius.data_ptr()
         lr_mean = self._fill_schedule(a, median_scale)

@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define BG_ABI_VERSION 9u
+#define BG_ABI_VERSION 10u
 
 /* f32 lanes per projected splat: a 64-byte row, four aligned 128-bit loads.  Lanes 0..8 are the reference
  * layout (kernels/helpers.rs:49-53: xy_x, xy_y, conic_x, conic_y, conic_z, color_a, color_r, color_g, color_b).
@@ -263,7 +263,12 @@ int32_t bg_train_step_depth(BgContext *ctx, void *stream, BgTrainStepArgs *args,
  * tensors (brush-train/src/adam_scaled.rs:75-165, train.rs:328-381), RefineRecord::gather_stats (stats.rs:40-50) and the
  * mean noise (train.rs:389-416; the draw is bg_normal_noise(seed, (step-1)*ceil(3n/4) ..)).  Gradients are the dense
  * outputs of bg_project_backward; v_refine / visible / max_radius are the step's statistics.  bg_train_step and
- * bg_train_step_views end with this pass; it is exported for hosts that drive the operators themselves. */
+ * bg_train_step_views end with this pass; it is exported for hosts that drive the operators themselves.
+ * The noise of a Gaussian is clamp(z * w * noise_scale, +-median_scale) with w = (1 - opacity)^150 where visible > 0
+ * and 0 elsewhere; opacity is taken after the update, sigmoid(raw_opac) or, with min_scale set (the 3D-filter floor
+ * of the step, as passed to bg_fold_min_scale_forward), the folded clamp(sigmoid(raw_opac) * coef, 1e-6, 1 - 1e-6)
+ * of Splats::opacities (gaussian_splats.rs:215-223).  transforms, m_t, v_t and v_transforms must be 8-byte aligned,
+ * sh, m_sh and v_sh_grad 16-byte aligned (else BG_ERR_INVALID, nothing written). */
 typedef struct {
     uint32_t n, k;
     float *transforms, *sh, *raw_opac;              /* [n,10] [n,k,3] [n], updated in place */
@@ -275,6 +280,7 @@ typedef struct {
     float noise_scale, median_scale;
     uint64_t seed;
     int32_t step;                                   /* 1-based Adam step; step == 1 initialises the moments */
+    const float *min_scale;                         /* [n] 3D-filter floor, or null: gates the noise on the folded opacity */
 } BgTrainUpdateArgs;
 int32_t bg_train_update(BgContext *ctx, void *stream, const BgTrainUpdateArgs *args);
 
@@ -551,7 +557,9 @@ int32_t bg_adam_step(BgContext *ctx, void *stream, float *p, const float *g, flo
 
 /* Replaces RefineRecord::gather_stats (brush-train/src/stats.rs:40-50) and the mean-noise update
  * (brush-train/src/train.rs:389-416) in one pass over the Gaussians.  noise: device [n,3] standard
- * normal draws (null skips the noise update). */
+ * normal draws (null skips the noise update); the weight is (1 - sigmoid(raw_opac))^150 * visible.  raw_opac is the
+ * opacity the reference gates on: with a 3D-filter floor, pass the folded raw opacity (raw_opac_out of
+ * bg_fold_min_scale_forward on the updated parameters), as bg_train_update does with its min_scale. */
 int32_t bg_refine_stats_noise(BgContext *ctx, void *stream, uint32_t n, const float *v_refine,
                               const float *visible, const float *max_radius, float *refine_weight_norm,
                               float *vis_weight, float *max_screen_size, float *transforms,
