@@ -16,7 +16,7 @@ BG_OK, BG_ERR_NULL, BG_ERR_INVALID, BG_ERR_CUDA, BG_ERR_CAPACITY, BG_ERR_UNSUPPO
 PASS_FORWARD, PASS_BACKWARD, PASS_BACKWARD_SMOOTH = 0, 1, 2
 PROJECTED_STRIDE = 16
 VCOMBINED_STRIDE = 10
-ABI_VERSION = 10
+ABI_VERSION = 11
 
 _STATUS_NAMES = {1: "BG_ERR_NULL", 2: "BG_ERR_INVALID", 3: "BG_ERR_CUDA", 4: "BG_ERR_CAPACITY", 5: "BG_ERR_UNSUPPORTED"}
 
@@ -164,6 +164,14 @@ class BgCompressArgs(C.Structure):
     ]
 
 
+class BgTsdfGrid(C.Structure):
+    _fields_ = [
+        ("origin", C.c_float * 3), ("h", C.c_float),
+        ("dims", C.c_uint32 * 3), ("trunc", C.c_float),
+        ("tsdf", C.c_void_p), ("weight", C.c_void_p), ("rgb", C.c_void_p),
+    ]
+
+
 class BgTrainViewsArgs(C.Structure):
     _fields_ = [
         ("w", C.c_uint32), ("h", C.c_uint32), ("n", C.c_uint32), ("k", C.c_uint32),
@@ -255,6 +263,10 @@ SIGNATURES = {
     "bg_decimate_to_count": (_I32, [_P, _P, C.POINTER(BgDecimateArgs)]),
     "bg_compress_workspace_bytes": (_U64, [_U32]),
     "bg_compress_splats": (_I32, [_P, _P, C.POINTER(BgCompressArgs)]),
+    "bg_tsdf_integrate": (_I32, [_P, _P, C.POINTER(BgTsdfGrid), C.POINTER(BgCamera), _U32, _U32, _P, _P, C.c_float]),
+    "bg_mesh_workspace_bytes": (_U64, [_U32, _U32, _U32]),
+    "bg_mesh_count": (_I32, [_P, _P, C.POINTER(BgTsdfGrid), _P, _U64, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
+    "bg_mesh_emit": (_I32, [_P, _P, C.POINTER(BgTsdfGrid), _P, _U64, _U32, _U32, _P, _P, _P]),
 }
 
 _lib = None

@@ -36,6 +36,7 @@ SOURCES = {
     "lod.cu": ["-fmad=false"],
     "depth_loss.cu": ["-fmad=false"],
     "compress.cu": ["-fmad=false"],
+    "mesh.cu": ["-fmad=false"],
 }
 
 

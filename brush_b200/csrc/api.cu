@@ -82,6 +82,14 @@ cudaError_t launch_compress_valid_bounds(cudaStream_t, uint32_t, uint32_t, const
 cudaError_t launch_compress_keys(cudaStream_t, uint32_t, const float *, const uint32_t *, uint32_t *, uint32_t *);
 cudaError_t launch_compress_chunks(cudaStream_t, uint32_t, uint32_t, const float *, const float *, const float *,
                                    const uint32_t *, const uint32_t *, float *, uint32_t *, uint8_t *, uint32_t *, uint32_t *);
+// mesh.cu
+cudaError_t launch_tsdf_integrate(cudaStream_t, const BgTsdfGrid &, const BgCamera &, uint32_t, uint32_t, const float *,
+                                  const float *, float);
+uint32_t mesh_num_bricks(const uint32_t *);
+cudaError_t launch_mesh_count(cudaStream_t, const BgTsdfGrid &, uint32_t *, uint32_t *, uint32_t *, uint32_t *,
+                              unsigned long long *);
+cudaError_t launch_mesh_emit(cudaStream_t, const BgTsdfGrid &, const uint32_t *, const uint32_t *, uint32_t *, uint8_t *,
+                             uint32_t, uint32_t, float *, uint8_t *, uint32_t *);
 // depth_loss.cu
 uint32_t depth_loss_num_partials(uint32_t, uint32_t);
 cudaError_t launch_depth_loss_fused(cudaStream_t, const float *, const float *, const float *, uint32_t, uint32_t, float, float *,
@@ -1462,5 +1470,118 @@ extern "C" int32_t bg_compress_splats(BgContext *c, void *stream, const BgCompre
     if (r != BG_OK) return r;
     BG_CUDA(launch_compress_chunks(s, n, k, a->transforms, a->sh, a->raw_opac, w.bounds, w.vals_s, a->chunks_out, a->packed_out,
                                    a->sh_out, a->order_out, a->count_out));
+    return BG_OK;
+}
+
+// ---- Mesh export (mesh.cu, DESIGN.md section 4.9)
+namespace {
+struct MeshWs {
+    unsigned long long *header;   // [8]: vertex total, triangle total, dims of the counted grid
+    uint32_t *brick_v, *brick_t, *voff, *toff, *vbase;
+    uint8_t *vmask;
+    uint64_t bytes;
+};
+MeshWs carve_mesh_ws(void *base, const uint32_t *dims) {
+    Carver cv{base};
+    MeshWs w;
+    const uint64_t nb = mesh_num_bricks(dims), np = (uint64_t)dims[0] * dims[1] * dims[2];
+    w.header = cv.take<unsigned long long>(8);
+    w.brick_v = cv.take<uint32_t>(nb); w.brick_t = cv.take<uint32_t>(nb);
+    w.voff = cv.take<uint32_t>(nb); w.toff = cv.take<uint32_t>(nb);
+    w.vbase = cv.take<uint32_t>(np);
+    w.vmask = cv.take<uint8_t>(np);
+    w.bytes = cv.off;
+    return w;
+}
+// Grid checks shared by the three calls: BG_OK, or the status with the message set.
+int32_t check_grid(const BgTsdfGrid *g, const char *who) {
+    char m[160];
+    if (!g->tsdf || !g->weight || !g->rgb) return BG_ERR_NULL;
+    const uint64_t np = (uint64_t)g->dims[0] * g->dims[1] * g->dims[2];
+    if (np == 0 || np >= (1ull << 31)) { snprintf(m, sizeof(m), "%s: grid dims must be non-zero with dx*dy*dz < 2^31", who); set_err(m, cudaSuccess); return BG_ERR_INVALID; }
+    if (((uintptr_t)g->tsdf | (uintptr_t)g->weight | (uintptr_t)g->rgb) % 4) { snprintf(m, sizeof(m), "%s: grid arrays must be 4-byte aligned", who); set_err(m, cudaSuccess); return BG_ERR_INVALID; }
+    if (!(g->h > 0.0f) || !std::isfinite(g->h) || !(g->trunc > 0.0f) || !std::isfinite(g->trunc) || !std::isfinite(g->origin[0]) ||
+        !std::isfinite(g->origin[1]) || !std::isfinite(g->origin[2])) {
+        snprintf(m, sizeof(m), "%s: grid origin must be finite, h and trunc finite and > 0", who); set_err(m, cudaSuccess); return BG_ERR_INVALID;
+    }
+    return BG_OK;
+}
+}  // namespace
+
+extern "C" int32_t bg_tsdf_integrate(BgContext *c, void *stream, const BgTsdfGrid *g, const BgCamera *cam, uint32_t w, uint32_t h,
+                                     const float *out_img, const float *out_depth, float alpha_min) {
+    if (!c || !g || !cam || !out_img || !out_depth) return BG_ERR_NULL;
+    int32_t r = check_grid(g, "bg_tsdf_integrate");
+    if (r != BG_OK) return r;
+    if (w == 0 || h == 0) { set_err("bg_tsdf_integrate: empty image", cudaSuccess); return BG_ERR_INVALID; }
+    if (!(alpha_min > 0.0f && alpha_min <= 1.0f)) { set_err("bg_tsdf_integrate: alpha_min must be in (0, 1]", cudaSuccess); return BG_ERR_INVALID; }
+    if (cam->camera_model > BG_CAMERA_THIN_PRISM_FISHEYE) { set_err("bg_tsdf_integrate: unknown camera model", cudaSuccess); return BG_ERR_INVALID; }
+    if ((uintptr_t)out_img % 16 || (uintptr_t)out_depth % 4) {
+        set_err("bg_tsdf_integrate: out_img must be 16-byte aligned, out_depth 4-byte", cudaSuccess);
+        return BG_ERR_INVALID;
+    }
+    BG_CUDA(cudaSetDevice(c->device));
+    BG_CUDA(launch_tsdf_integrate((cudaStream_t)stream, *g, *cam, w, h, out_img, out_depth, alpha_min));
+    return BG_OK;
+}
+
+extern "C" uint64_t bg_mesh_workspace_bytes(uint32_t dx, uint32_t dy, uint32_t dz) {
+    const uint32_t dims[3] = {std::max(dx, 1u), std::max(dy, 1u), std::max(dz, 1u)};
+    return carve_mesh_ws(nullptr, dims).bytes;
+}
+
+namespace {
+int32_t mesh_ws_for(const BgTsdfGrid *g, void *ws, uint64_t ws_bytes, const char *who, MeshWs &w) {
+    char m[160];
+    if (!ws) return BG_ERR_NULL;
+    if ((uintptr_t)ws % 256) { snprintf(m, sizeof(m), "%s: workspace must be 256-byte aligned", who); set_err(m, cudaSuccess); return BG_ERR_INVALID; }
+    w = carve_mesh_ws(ws, g->dims);
+    if (w.bytes > ws_bytes) { snprintf(m, sizeof(m), "%s: workspace too small (bg_mesh_workspace_bytes)", who); set_err(m, cudaSuccess); return BG_ERR_CAPACITY; }
+    return BG_OK;
+}
+}  // namespace
+
+extern "C" int32_t bg_mesh_count(BgContext *c, void *stream, const BgTsdfGrid *g, void *ws, uint64_t ws_bytes, uint32_t *num_vertices,
+                                 uint32_t *num_triangles) {
+    if (!c || !g || !num_vertices || !num_triangles) return BG_ERR_NULL;
+    *num_vertices = 0;
+    *num_triangles = 0;
+    int32_t r = check_grid(g, "bg_mesh_count");
+    if (r != BG_OK) return r;
+    MeshWs w;
+    if ((r = mesh_ws_for(g, ws, ws_bytes, "bg_mesh_count", w)) != BG_OK) return r;
+    cudaStream_t s = (cudaStream_t)stream;
+    BG_CUDA(cudaSetDevice(c->device));
+    BG_CUDA(launch_mesh_count(s, *g, w.brick_v, w.brick_t, w.voff, w.toff, w.header));
+    unsigned long long host[2];
+    BG_CUDA(cudaMemcpyAsync(host, w.header, sizeof(host), cudaMemcpyDeviceToHost, s));
+    BG_CUDA(cudaStreamSynchronize(s));
+    if (host[0] > 0xFFFFFFFFull || host[1] > 0xFFFFFFFFull) { set_err("bg_mesh_count: more than 2^32 - 1 vertices or triangles", cudaSuccess); return BG_ERR_CAPACITY; }
+    *num_vertices = (uint32_t)host[0];
+    *num_triangles = (uint32_t)host[1];
+    return BG_OK;
+}
+
+extern "C" int32_t bg_mesh_emit(BgContext *c, void *stream, const BgTsdfGrid *g, void *ws, uint64_t ws_bytes, uint32_t max_vertices,
+                                uint32_t max_triangles, float *vertices, uint8_t *colors, uint32_t *faces) {
+    if (!c || !g) return BG_ERR_NULL;
+    int32_t r = check_grid(g, "bg_mesh_emit");
+    if (r != BG_OK) return r;
+    if ((max_vertices && (!vertices || !colors)) || (max_triangles && !faces)) return BG_ERR_NULL;
+    if (((uintptr_t)vertices | (uintptr_t)faces) % 4) { set_err("bg_mesh_emit: vertices and faces must be 4-byte aligned", cudaSuccess); return BG_ERR_INVALID; }
+    MeshWs w;
+    if ((r = mesh_ws_for(g, ws, ws_bytes, "bg_mesh_emit", w)) != BG_OK) return r;
+    cudaStream_t s = (cudaStream_t)stream;
+    BG_CUDA(cudaSetDevice(c->device));
+    unsigned long long host[5];
+    BG_CUDA(cudaMemcpyAsync(host, w.header, sizeof(host), cudaMemcpyDeviceToHost, s));
+    BG_CUDA(cudaStreamSynchronize(s));
+    if (host[2] != g->dims[0] || host[3] != g->dims[1] || host[4] != g->dims[2]) {
+        set_err("bg_mesh_emit: the workspace holds no bg_mesh_count of a grid with these dims", cudaSuccess);
+        return BG_ERR_INVALID;
+    }
+    if (host[0] > max_vertices || host[1] > max_triangles) { set_err("bg_mesh_emit: the mesh exceeds max_vertices / max_triangles", cudaSuccess); return BG_ERR_CAPACITY; }
+    if (host[0] == 0) return BG_OK;   // no vertices, so no triangles
+    BG_CUDA(launch_mesh_emit(s, *g, w.voff, w.toff, w.vbase, w.vmask, max_vertices, max_triangles, vertices, colors, faces));
     return BG_OK;
 }

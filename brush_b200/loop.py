@@ -26,6 +26,8 @@ class ProcessConfig:                     # brush-process/src/config.rs (the fiel
     seed: int = 42
     eval_save_to_disk: bool = False     # the rendered eval images go to <export_path>/eval_<iter>/<image name>.png
     export_compressed: bool = False     # exports (every LOD level included) use the SuperSplat compressed layout
+    export_mesh: bool = False           # when the main run ends, also write <level-0 export name>_mesh.ply (DESIGN.md 4.9)
+    mesh_resolution: int = 512          # TSDF lattice points along the longest axis of the mesh bounds
 
 
 def should_refine(it: int, refine_every: int, total_iters: int) -> bool:
@@ -153,6 +155,13 @@ def train_loop(ctx, splats, train_views: Sequence, eval_views: Sequence, config,
         with open(os.path.join(process.export_path, name), "wb") as f:
             f.write(data)
 
+    def export_mesh(name: str):
+        from .mesh import splats_to_mesh                    # TSDF fusion of the training views (DESIGN.md section 4.9)
+        m = splats_to_mesh(ctx, splats, train_views, resolution=process.mesh_resolution, render_mip=config.render_mip)
+        os.makedirs(process.export_path, exist_ok=True)
+        with open(os.path.join(process.export_path, name), "wb") as f:
+            f.write(m.to_ply())
+
     for it in range(process.start_iter, total_all):
         target = lod_level(it, total, config.lod_levels, steps)
         if target > level:                                  # train_stream.rs:227-291
@@ -200,6 +209,9 @@ def train_loop(ctx, splats, train_views: Sequence, eval_views: Sequence, config,
             evals.append(rec)
         if should_export_lod(done, level, process.export_every, total_all, config.lod_levels):
             export(lod_export_name(process.export_name, level, done, steps))
+        if process.export_mesh and level == 0 and done == total:
+            check_overflow()
+            export_mesh(lod_export_name(process.export_name, 0, done, steps).replace(".ply", "_mesh.ply"))
     torch.cuda.synchronize(ctx.device)
     check_overflow()
     loader.close()

@@ -402,3 +402,23 @@ def compressed_ply_bytes(chunks: np.ndarray, packed: np.ndarray, sh_bytes: Optio
         head += [f"element sh {m}"] + [f"property uchar f_rest_{i}" for i in range(rest)]
         body += np.ascontiguousarray(sh_bytes[:m], np.uint8).tobytes()
     return ("\n".join(head + ["end_header"]) + "\n").encode("ascii") + body
+
+
+def mesh_to_ply(vertices: np.ndarray, colors: np.ndarray, faces: np.ndarray) -> bytes:
+    """A coloured triangle mesh (DESIGN.md section 4.9) as binary little-endian PLY: vertex x, y, z (float) and red, green,
+    blue (uchar); face vertex_indices (list uchar int, three per face)."""
+    v = np.ascontiguousarray(vertices, np.float32).reshape(-1, 3)
+    c = np.ascontiguousarray(colors, np.uint8).reshape(-1, 3)
+    f = np.asarray(faces).reshape(-1, 3)
+    if len(c) != len(v):
+        raise ValueError("mesh_to_ply: one colour per vertex")
+    if len(f) and (f.min() < 0 or f.max() >= len(v)):
+        raise ValueError("mesh_to_ply: face index out of range")
+    head = ["ply", "format binary_little_endian 1.0", f"element vertex {len(v)}", "property float x", "property float y",
+            "property float z", "property uchar red", "property uchar green", "property uchar blue",
+            f"element face {len(f)}", "property list uchar int vertex_indices", "end_header"]
+    vrow = np.empty(len(v), np.dtype([("p", "<f4", 3), ("c", "u1", 3)]))
+    vrow["p"], vrow["c"] = v, c
+    frow = np.empty(len(f), np.dtype([("n", "u1"), ("i", "<i4", 3)]))
+    frow["n"], frow["i"] = 3, f
+    return ("\n".join(head) + "\n").encode("ascii") + vrow.tobytes() + frow.tobytes()

@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define BG_ABI_VERSION 10u
+#define BG_ABI_VERSION 11u
 
 /* f32 lanes per projected splat: a 64-byte row, four aligned 128-bit loads.  Lanes 0..8 are the reference
  * layout (kernels/helpers.rs:49-53: xy_x, xy_y, conic_x, conic_y, conic_z, color_a, color_r, color_g, color_b).
@@ -404,6 +404,40 @@ typedef struct {
 } BgCompressArgs;
 uint64_t bg_compress_workspace_bytes(uint32_t n);
 int32_t bg_compress_splats(BgContext *ctx, void *stream, const BgCompressArgs *args);
+
+/* ---- Mesh export (DESIGN.md section 4.9; no reference operator): fuse rendered depth into a truncated signed distance
+ * field (TSDF) on a dense lattice, then extract its zero level set as a coloured triangle mesh.
+ * The grid is dims[0] x dims[1] x dims[2] points (dx * dy * dz < 2^31), x fastest ([dz, dy, dx]); point (i, j, k) sits at
+ * origin + (float(i), float(j), float(k)) * h.  Per point: f32 tsdf, f32 weight, f32 rgb[3] (20 bytes), allocated and
+ * zeroed by the caller; weight == 0 means unobserved.  Arrays 4-byte aligned.
+ * bg_tsdf_integrate fuses one view: out_img [h,w,4] and out_depth [h,w] from bg_render_forward_depth on a BLACK
+ *     background (16- and 4-byte aligned), cam the render's camera (any of the four models).  A point is updated when
+ *     z = (viewmat x)_z >= 0.01 and finite, its projection (u, v) satisfies 0 <= u < w and 0 <= v < h, the pixel
+ *     (floor u, floor v) has a = out_img[..,3] >= alpha_min, ed = D / a is finite and > 0, and sdf = ed - z >= -trunc:
+ *     then with f = min(1, sdf / trunc) and c = clamp(rgb / a, 0, 1), W' = W + 1, T' = (T W + f) / W', C' = (C W + c) / W'.
+ *     Points not updated are neither read nor written.  0 < alpha_min <= 1, h > 0, trunc > 0, else BG_ERR_INVALID.
+ * bg_mesh_count (blocking: one readback) runs marching tetrahedra over the 6 Kuhn tetrahedra of every cell and returns the
+ *     vertex and triangle counts in host scalars; counts beyond 2^32 - 1 return BG_ERR_CAPACITY.  The workspace keeps the
+ *     per-brick offsets for bg_mesh_emit, which writes vertices [V,3] f32, colors [V,3] u8 and faces [F,3] u32 in the
+ *     deterministic order of DESIGN.md section 4.9.  The grid must not change between the two calls; emit reads the counts
+ *     back once and returns BG_ERR_CAPACITY, writing nothing, when V > max_vertices or F > max_triangles.  Workspace:
+ *     bg_mesh_workspace_bytes(dims), 256-byte aligned. */
+typedef struct {
+    float origin[3];
+    float h;                    /* lattice spacing */
+    uint32_t dims[3];           /* dx, dy, dz */
+    float trunc;                /* truncation distance, scene units */
+    float *tsdf;                /* [dz, dy, dx] */
+    float *weight;              /* [dz, dy, dx] */
+    float *rgb;                 /* [dz, dy, dx, 3] */
+} BgTsdfGrid;
+int32_t bg_tsdf_integrate(BgContext *ctx, void *stream, const BgTsdfGrid *grid, const BgCamera *cam, uint32_t w,
+                          uint32_t h, const float *out_img, const float *out_depth, float alpha_min);
+uint64_t bg_mesh_workspace_bytes(uint32_t dx, uint32_t dy, uint32_t dz);
+int32_t bg_mesh_count(BgContext *ctx, void *stream, const BgTsdfGrid *grid, void *workspace, uint64_t workspace_bytes,
+                      uint32_t *num_vertices /* host */, uint32_t *num_triangles /* host */);
+int32_t bg_mesh_emit(BgContext *ctx, void *stream, const BgTsdfGrid *grid, void *workspace, uint64_t workspace_bytes,
+                     uint32_t max_vertices, uint32_t max_triangles, float *vertices, uint8_t *colors, uint32_t *faces);
 
 /* ---- View-sharded data parallelism behind the boundary (SURVEY.md section 8e; the reference is single-device).
  * A communicator is one NCCL rank bound to the context's device.  Rank 0 calls bg_dp_unique_id and ships the 128 bytes

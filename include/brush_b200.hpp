@@ -20,6 +20,8 @@
 //   pup_scores, decimate_to_count <- LOD baking, brush-train/src/lod.rs:13-142 (bg_pup_*, bg_decimate_to_count)
 //   compress_splats, compressed_ply_bytes <- SuperSplat compressed PLY export (bg_compress_splats; the reference only reads
 //                                  the layout, brush-serde/src/import.rs:408-600)
+//   TsdfGrid, tsdf_integrate, extract_mesh, mesh_ply_bytes <- mesh export (bg_tsdf_integrate, bg_mesh_count, bg_mesh_emit;
+//                                  no reference counterpart, DESIGN.md section 4.9)
 //
 // Errors: the reference panics on shape / device violations (render.rs:50-64); here every non-zero ABI status
 // becomes a brush_b200::Error (std::runtime_error) carrying the status and bg_last_error_string().
@@ -924,6 +926,74 @@ inline std::string compressed_ply_bytes(const CompressedSplats &c, const std::ve
     s.append(reinterpret_cast<const char *>(c.chunks.data()), (size_t)n_chunks * 18 * sizeof(float));
     s.append(reinterpret_cast<const char *>(c.packed.data()), (size_t)m * 4 * sizeof(uint32_t));
     if (rest) s.append(reinterpret_cast<const char *>(c.sh.data()), (size_t)m * rest);
+    return s;
+}
+
+// ---------------------------------------------------------------------------------------------- mesh export
+// A dense TSDF grid on the device (DESIGN.md section 4.9), zeroed (unobserved) at construction: dims[0] x dims[1] x dims[2]
+// points at origin + (i, j, k) * h, truncation `trunc`.
+struct TsdfGrid {
+    BgTsdfGrid grid;
+    DeviceBuffer<float> tsdf, weight, rgb;
+    TsdfGrid(const float origin[3], float h, const uint32_t dims[3], float trunc) {
+        const uint64_t n = (uint64_t)dims[0] * dims[1] * dims[2];
+        if (n == 0 || n >= (1ull << 31)) throw Error(BG_ERR_INVALID, "TsdfGrid: dims must be non-zero with dx*dy*dz < 2^31");
+        tsdf = DeviceBuffer<float>(n, true);
+        weight = DeviceBuffer<float>(n, true);
+        rgb = DeviceBuffer<float>(n * 3, true);
+        std::memset(&grid, 0, sizeof(grid));
+        for (int a = 0; a < 3; a++) { grid.origin[a] = origin[a]; grid.dims[a] = dims[a]; }
+        grid.h = h;
+        grid.trunc = trunc;
+        grid.tsdf = tsdf.data(); grid.weight = weight.data(); grid.rgb = rgb.data();
+    }
+};
+
+// Fuses one view: out_img [h,w,4] and out_depth [h,w] of render_splats_depth on a black background, cam its uniforms.
+inline void tsdf_integrate(Context &ctx, cudaStream_t stream, TsdfGrid &g, const BgCamera &cam, uint32_t w, uint32_t h,
+                           const float *out_img, const float *out_depth, float alpha_min = 0.5f) {
+    check(bg_tsdf_integrate(ctx.handle(), stream, &g.grid, &cam, w, h, out_img, out_depth, alpha_min), "tsdf_integrate");
+}
+
+struct TriangleMesh {
+    std::vector<float> vertices;     // [V, 3]
+    std::vector<uint8_t> colors;     // [V, 3]
+    std::vector<uint32_t> faces;     // [F, 3], normals toward free space
+};
+
+// Marching tetrahedra over the grid: one count readback, then the vertices, colours and faces copied to the host.
+inline TriangleMesh extract_mesh(Context &ctx, cudaStream_t stream, const TsdfGrid &g) {
+    const uint64_t need = bg_mesh_workspace_bytes(g.grid.dims[0], g.grid.dims[1], g.grid.dims[2]);
+    DeviceBuffer<unsigned char> ws(need);
+    uint32_t nv = 0, nt = 0;
+    check(bg_mesh_count(ctx.handle(), stream, &g.grid, ws.data(), need, &nv, &nt), "extract_mesh: count");
+    DeviceBuffer<float> v((size_t)nv * 3);
+    DeviceBuffer<uint8_t> c((size_t)nv * 3);
+    DeviceBuffer<uint32_t> f((size_t)nt * 3);
+    check(bg_mesh_emit(ctx.handle(), stream, &g.grid, ws.data(), need, nv, nt, v.data(), c.data(), f.data()), "extract_mesh: emit");
+    TriangleMesh m;
+    m.vertices.resize((size_t)nv * 3); m.colors.resize((size_t)nv * 3); m.faces.resize((size_t)nt * 3);
+    if (nv) { v.download(m.vertices.data(), m.vertices.size(), stream); c.download(m.colors.data(), m.colors.size(), stream); }
+    if (nt) f.download(m.faces.data(), m.faces.size(), stream);
+    return m;
+}
+
+// The file bytes, identical to brush_b200.ply.mesh_to_ply (binary little-endian; this header assumes a little-endian host).
+inline std::string mesh_ply_bytes(const TriangleMesh &m) {
+    const size_t nv = m.vertices.size() / 3, nf = m.faces.size() / 3;
+    std::string s = "ply\nformat binary_little_endian 1.0\nelement vertex " + std::to_string(nv) +
+                    "\nproperty float x\nproperty float y\nproperty float z\nproperty uchar red\nproperty uchar green\n"
+                    "property uchar blue\nelement face " + std::to_string(nf) +
+                    "\nproperty list uchar int vertex_indices\nend_header\n";
+    s.reserve(s.size() + nv * 15 + nf * 13);
+    for (size_t i = 0; i < nv; i++) {
+        s.append(reinterpret_cast<const char *>(&m.vertices[i * 3]), 12);
+        s.append(reinterpret_cast<const char *>(&m.colors[i * 3]), 3);
+    }
+    for (size_t i = 0; i < nf; i++) {
+        s.push_back((char)3);
+        s.append(reinterpret_cast<const char *>(&m.faces[i * 3]), 12);
+    }
     return s;
 }
 
