@@ -15,87 +15,7 @@
 #include "bg_dp.cuh"
 #include "bg_update.cuh"
 #include "bg_refine.cuh"
-
-namespace bg {
-// project.cu
-cudaError_t launch_project_cull(cudaStream_t, int, bool, int, const float *, const float *, const float *, uint32_t,
-                                const BgCamera &, uint32_t, uint32_t, uint32_t, uint32_t, uint32_t *, uint32_t *,
-                                uint32_t *, float *, uint32_t *, float *, uint32_t *, unsigned long long *,
-                                const uint32_t *, uint32_t);
-cudaError_t launch_gather_scan(cudaStream_t, int, const uint32_t *, const uint32_t *, uint32_t, const uint32_t *,
-                               uint32_t *, uint32_t *, uint32_t, uint32_t *, uint32_t *, unsigned long long *,
-                               const uint32_t *, uint32_t);
-cudaError_t launch_project_visible_emit(cudaStream_t, int, const float *, const uint32_t *, const uint32_t *, uint32_t,
-                                        uint32_t, float *, uint32_t *, uint32_t *, uint32_t, uint32_t *, uint32_t *,
-                                        uint32_t);
-cudaError_t launch_tile_offsets(cudaStream_t, int, const uint32_t *, const uint32_t *, uint32_t, uint32_t *);
-// sort.cu
-cudaError_t launch_radix_hist(cudaStream_t, int, const uint32_t *, uint32_t, const uint32_t *, uint32_t, uint32_t,
-                              uint32_t *);
-cudaError_t launch_onesweep_pass(cudaStream_t, int, const uint32_t *, const uint32_t *, uint32_t *, uint32_t *,
-                                 uint32_t, const uint32_t *, uint32_t, uint32_t, const uint32_t *, uint32_t *,
-                                 unsigned long long *, unsigned long long *, const uint32_t *, uint32_t);
-cudaError_t launch_bump_epoch(cudaStream_t, uint32_t *);
-uint64_t sort_max_tiles(uint64_t n);
-// blend_fwd.cu / blend_bwd.cu
-cudaError_t launch_blend_fwd(cudaStream_t, bool, bool, uint32_t, const float *, const uint32_t *, uint32_t *, const uint32_t *,
-                             void *, float *, uint32_t *, uint32_t *, uint32_t, uint32_t, uint32_t, const float *, const float *,
-                             float *);
-cudaError_t launch_blend_bwd(cudaStream_t, bool, uint32_t, const float *, const uint32_t *, const uint32_t *, const float *,
-                             const float *, const uint32_t *, const uint32_t *, float *, unsigned long long *, uint32_t,
-                             uint32_t, uint32_t, const float *, const float *, const float *, const float *, float *);
-// project_bwd.cu
-cudaError_t launch_project_bwd(cudaStream_t, bool, int, const float *, const float *, const float *,
-                               const uint32_t *, const float *, uint32_t, const BgCamera &, float *, float *, float *,
-                               float *, float *);
-cudaError_t launch_depth_to_means(cudaStream_t, const uint32_t *, const float *, uint32_t, const BgCamera &, float *);
-cudaError_t launch_normal_noise(cudaStream_t, uint64_t, uint64_t, uint64_t, float *);
-cudaError_t launch_loss_reduce(cudaStream_t, const float *, uint32_t, uint32_t, const float *, float *);
-cudaError_t launch_min_scale(cudaStream_t, uint32_t, const float *, const float *, uint32_t, float, float *);
-cudaError_t launch_fold_min_scale_fwd(cudaStream_t, uint32_t, const float *, const float *, const float *, float *, float *);
-cudaError_t launch_fold_min_scale_bwd(cudaStream_t, uint32_t, const float *, const float *, const float *, float *, float *);
-cudaError_t launch_fold_min_scale_bwd_strided(cudaStream_t, uint32_t, const float *, const float *, const float *, float *, float *,
-                                              uint32_t, uint32_t);
-cudaError_t launch_sh_grad_from_views(cudaStream_t, int, const float *, const float *, uint32_t, const float *, uint32_t,
-                                      float, float *, size_t);
-// loss.cu / optim.cu
-cudaError_t launch_image_loss_fwd(cudaStream_t, const float *, const uint32_t *, uint32_t, uint32_t, uint32_t, int64_t,
-                                  int64_t, int64_t, float, float, const float *, bool, float *);
-cudaError_t launch_image_loss_bwd(cudaStream_t, const float *, const uint32_t *, const float *, uint32_t, uint32_t,
-                                  uint32_t, int64_t, int64_t, int64_t, float, float, const float *, bool, float *);
-cudaError_t launch_image_loss_fused(cudaStream_t, const float *, const uint32_t *, uint32_t, uint32_t, uint32_t, int64_t,
-                                    int64_t, int64_t, float, float, const float *, bool, const float *, float *, float *);
-uint32_t image_loss_fused_num_partials(uint32_t, uint32_t, uint32_t);
-cudaError_t launch_adam(cudaStream_t, float *, const float *, float *, float *, uint64_t, uint32_t, const float *, float,
-                        float, float, float, float, float, bool, bool);
-cudaError_t launch_refine_stats_noise(cudaStream_t, uint32_t, const float *, const float *, const float *, float *,
-                                      float *, float *, float *, const float *, const float *, float, float);
-// lod.cu
-cudaError_t launch_pup_accumulate(cudaStream_t, uint32_t, const float *, bool, float *);
-cudaError_t launch_pup_log_det(cudaStream_t, uint32_t, const float *, float *);
-cudaError_t launch_decimate_keys(cudaStream_t, uint32_t, const float *, uint32_t *, uint32_t *);
-cudaError_t launch_decimate_gather(cudaStream_t, uint32_t, uint32_t, const uint32_t *, const float *, const float *,
-                                   const float *, const float *, float *, float *, float *, float *);
-// compress.cu
-cudaError_t launch_compress_valid_bounds(cudaStream_t, uint32_t, uint32_t, const float *, const float *, const float *,
-                                         uint32_t *, uint32_t *);
-cudaError_t launch_compress_keys(cudaStream_t, uint32_t, const float *, const uint32_t *, uint32_t *, uint32_t *);
-cudaError_t launch_compress_chunks(cudaStream_t, uint32_t, uint32_t, const float *, const float *, const float *,
-                                   const uint32_t *, const uint32_t *, float *, uint32_t *, uint8_t *, uint32_t *, uint32_t *);
-// mesh.cu
-cudaError_t launch_tsdf_integrate(cudaStream_t, const BgTsdfGrid &, const BgCamera &, uint32_t, uint32_t, const float *,
-                                  const float *, float);
-uint32_t mesh_num_bricks(const uint32_t *);
-cudaError_t launch_mesh_count(cudaStream_t, const BgTsdfGrid &, uint32_t *, uint32_t *, uint32_t *, uint32_t *,
-                              unsigned long long *);
-cudaError_t launch_mesh_emit(cudaStream_t, const BgTsdfGrid &, const uint32_t *, const uint32_t *, uint32_t *, uint8_t *,
-                             uint32_t, uint32_t, float *, uint8_t *, uint32_t *);
-// depth_loss.cu
-uint32_t depth_loss_num_partials(uint32_t, uint32_t);
-cudaError_t launch_depth_loss_fused(cudaStream_t, const float *, const float *, const float *, uint32_t, uint32_t, float, float *,
-                                    float *, float *);
-cudaError_t launch_depth_loss_reduce(cudaStream_t, const float *, uint32_t, float, float *, float *);
-}  // namespace bg
+#include "bg_launch.cuh"
 
 using namespace bg;
 
@@ -112,6 +32,44 @@ static void set_err(const char *what, cudaError_t e) {
             return BG_ERR_CUDA;                \
         }                                      \
     } while (0)
+
+// ---- argument checks shared by the entry points.  Each returns BG_OK or the status, with the error text set.
+// The text is "who: what", or "who what" when `what` opens with a space.
+static int32_t fail(int32_t status, const char *who, const char *what) {
+    char m[480];
+    snprintf(m, sizeof(m), what[0] == ' ' ? "%s%s" : "%s: %s", who, what);
+    set_err(m, cudaSuccess);
+    return status;
+}
+static int32_t invalid(const char *who, const char *what) { return fail(BG_ERR_INVALID, who, what); }
+static int32_t capacity(const char *who, const char *what) { return fail(BG_ERR_CAPACITY, who, what); }
+
+// k SH coefficients per channel must be (deg + 1)^2 with deg <= 4; *deg gets the degree
+static int32_t check_k(uint32_t k, int *deg = nullptr) {
+    const int d = sh_degree_from_k(k);
+    if (deg) *deg = d;
+    if (d < 0) set_err("Invalid nr. of sh bases", cudaSuccess);
+    return d < 0 ? BG_ERR_INVALID : BG_OK;
+}
+
+// A caller-provided workspace: non-null and 256-byte aligned (what Carver's blocks assume), and at least `need` bytes,
+// the figure that the function named `sizer` reports.  In two parts for the entry points that check other arguments
+// in between.
+static int32_t check_workspace_aligned(const char *who, const void *ws) {
+    if (!ws) return BG_ERR_NULL;
+    if ((uintptr_t)ws % 256) return invalid(who, "workspace must be 256-byte aligned");
+    return BG_OK;
+}
+static int32_t check_workspace_bytes(const char *who, const char *sizer, uint64_t have, uint64_t need) {
+    if (need <= have) return BG_OK;
+    char what[96];
+    snprintf(what, sizeof(what), "workspace too small (%s)", sizer);
+    return capacity(who, what);
+}
+static int32_t check_workspace(const char *who, const char *sizer, const void *ws, uint64_t have, uint64_t need) {
+    if (int32_t r = check_workspace_aligned(who, ws); r != BG_OK) return r;
+    return check_workspace_bytes(who, sizer, have, need);
+}
 
 struct BgContext {
     int device = 0;
@@ -142,6 +100,9 @@ struct BgContext {
     int depth_out = 0, isect_out = 0;
     bool depth_forward = false;   // the last forward also accumulated depth (bg_render_forward_depth)
 };
+
+// The most keys the context's radix sort takes: its scratch is the larger of the depth and intersection ping-pong buffers.
+static uint32_t sort_capacity(const BgContext *c) { return std::max(c->max_n, c->max_isect); }
 
 // Launch indices inside one API call (each look-back chain of a call gets its own epoch).
 enum EpochSlots : uint32_t { EP_PROJECT = 0, EP_DEPTH_SORT = 1 /* ..4 */, EP_SCAN = 5, EP_TILE_SORT = 6 /* ..9 */ };
@@ -175,9 +136,9 @@ extern "C" int32_t bg_ctx_create(int32_t device, uint32_t max_splats, uint32_t m
                                  uint64_t max_intersections, BgContext **out_ctx) {
     if (!out_ctx) return BG_ERR_NULL;
     *out_ctx = nullptr;
-    if (max_splats == 0 || max_w == 0 || max_h == 0) { set_err("bg_ctx_create: zero capacity", cudaSuccess); return BG_ERR_INVALID; }
+    if (max_splats == 0 || max_w == 0 || max_h == 0) return invalid("bg_ctx_create", "zero capacity");
     if (max_intersections == 0) max_intersections = std::max<uint64_t>(16ull * max_splats, 1ull << 22);
-    if (max_intersections >= (1ull << 31)) { set_err("bg_ctx_create: max_intersections must be < 2^31", cudaSuccess); return BG_ERR_INVALID; }
+    if (max_intersections >= (1ull << 31)) return invalid("bg_ctx_create", "max_intersections must be < 2^31");
     BG_CUDA(cudaSetDevice(device));
     BgContext *c = new (std::nothrow) BgContext();
     if (!c) return BG_ERR_CUDA;
@@ -267,19 +228,17 @@ static int32_t render_forward(BgContext *c, void *stream, const BgCamera *cam, u
     if (n > 0 && !max_radius) return BG_ERR_NULL;
     if (n > 0 && (!transforms || !sh || !raw_opac)) return BG_ERR_NULL;
     if (w == 0 || h == 0) { set_err("Can't render images with 0 size", cudaSuccess); return BG_ERR_INVALID; }
-    const int deg = sh_degree_from_k(k);
-    if (deg < 0) { set_err("Invalid nr. of sh bases", cudaSuccess); return BG_ERR_INVALID; }
+    int deg;
+    if (int32_t r = check_k(k, &deg); r != BG_OK) return r;
     if (pass < 0 || pass > 2) { set_err("invalid pass", cudaSuccess); return BG_ERR_INVALID; }
     if (cam->camera_model > BG_CAMERA_THIN_PRISM_FISHEYE) return BG_ERR_UNSUPPORTED;
     const bool bwd_info = pass != BG_PASS_FORWARD;
     if (bwd_info && n > 0 && !visible) return BG_ERR_NULL;
-    if ((((uintptr_t)transforms) | ((uintptr_t)sh) | ((uintptr_t)raw_opac) | ((uintptr_t)out_img)) & 15u) {
-        set_err("bg_render_forward: arrays must be 16-byte aligned (bulk / 128-bit access)", cudaSuccess);
-        return BG_ERR_INVALID;
-    }
+    if ((((uintptr_t)transforms) | ((uintptr_t)sh) | ((uintptr_t)raw_opac) | ((uintptr_t)out_img)) & 15u)
+        return invalid("bg_render_forward", "arrays must be 16-byte aligned (bulk / 128-bit access)");
     const uint32_t tiles_x = (w + TILE_W - 1) / TILE_W, tiles_y = (h + TILE_W - 1) / TILE_W;
     const uint32_t num_tiles = tiles_x * tiles_y;
-    if (n > c->max_n || num_tiles > c->max_tiles) { set_err("bg_render_forward: exceeds context capacity", cudaSuccess); return BG_ERR_CAPACITY; }
+    if (n > c->max_n || num_tiles > c->max_tiles) return capacity("bg_render_forward", "exceeds context capacity");
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
     c->depth_forward = out_depth != nullptr;
@@ -319,13 +278,10 @@ static int32_t render_forward(BgContext *c, void *stream, const BgCamera *cam, u
                                             bits));
     int iout = 0;
     {
-        const uint32_t passes = (bits + 7) / 8;
-        const int first_dst = 1;
         int32_t r = run_sort(c, s, c->isect_key[0], c->isect_val[0], c->isect_key, c->isect_val, c->max_isect,
-                             counters + 1, bits, c->ctl + CTL_HIST_TILE, c->ctl + CTL_TICKETS + TK_TILE_HIST, first_dst,
+                             counters + 1, bits, c->ctl + CTL_HIST_TILE, c->ctl + CTL_TICKETS + TK_TILE_HIST, 1,
                              EP_TILE_SORT, &iout, /*hist_ready=*/n > 0 && bits <= 16);
         if (r != BG_OK) return r;
-        (void)passes;
     }
     c->isect_out = iout;
     // K4
@@ -364,11 +320,9 @@ extern "C" int32_t bg_render_forward_depth(BgContext *c, void *stream, const BgC
                                            float *out_img, float *out_depth, float *visible, float *max_radius,
                                            BgRenderState *st) {
     if (!out_depth) return BG_ERR_NULL;
-    if (pass != BG_PASS_BACKWARD && pass != BG_PASS_BACKWARD_SMOOTH) {
-        set_err("bg_render_forward_depth: depth needs an f32 pass (BG_PASS_BACKWARD or BG_PASS_BACKWARD_SMOOTH)", cudaSuccess);
-        return BG_ERR_INVALID;
-    }
-    if ((uintptr_t)out_depth % 4) { set_err("bg_render_forward_depth: out_depth must be 4-byte aligned", cudaSuccess); return BG_ERR_INVALID; }
+    if (pass != BG_PASS_BACKWARD && pass != BG_PASS_BACKWARD_SMOOTH)
+        return invalid("bg_render_forward_depth", "depth needs an f32 pass (BG_PASS_BACKWARD or BG_PASS_BACKWARD_SMOOTH)");
+    if ((uintptr_t)out_depth % 4) return invalid("bg_render_forward_depth", "out_depth must be 4-byte aligned");
     return render_forward(c, stream, cam, w, h, n, k, transforms, sh, raw_opac, mip, bg, pass, out_img, out_depth, visible,
                           max_radius, st);
 }
@@ -377,17 +331,11 @@ extern "C" int32_t bg_render_forward_depth(BgContext *c, void *stream, const BgC
 static int32_t rasterize_backward(BgContext *c, void *stream, const BgRenderState *st, const float *out_img,
                                   const float *out_depth, const float *v_output, const float *v_depth, const float *bg,
                                   int32_t smooth, float *v_combined, uint32_t rows, float *v_z, const char *who) {
-    auto invalid = [who](const char *what) {
-        char m[160];
-        snprintf(m, sizeof(m), "%s%s", who, what);
-        set_err(m, cudaSuccess);
-        return BG_ERR_INVALID;
-    };
-    if (st->pass == BG_PASS_FORWARD) return invalid(" requires a Backward pass state");
+    if (st->pass == BG_PASS_FORWARD) return invalid(who, " requires a Backward pass state");
     const bool smooth_pass = st->pass == BG_PASS_BACKWARD_SMOOTH;
-    if ((smooth != 0) != smooth_pass) return invalid(": smooth_cutoff must match the state's pass");
-    if (st->tile_offsets != c->tile_offsets) return invalid(": needs the state of this context's last forward");
-    if (v_z && !c->depth_forward) return invalid(": this context's last forward did not render depth");
+    if ((smooth != 0) != smooth_pass) return invalid(who, "smooth_cutoff must match the state's pass");
+    if (st->tile_offsets != c->tile_offsets) return invalid(who, "needs the state of this context's last forward");
+    if (v_z && !c->depth_forward) return invalid(who, "this context's last forward did not render depth");
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
     const uint32_t zr = std::min(rows, std::max(st->n, 1u));
@@ -413,10 +361,8 @@ extern "C" int32_t bg_rasterize_backward_depth(BgContext *c, void *stream, const
                                                const float *bg, int32_t smooth, float *v_combined, uint32_t rows,
                                                float *v_z) {
     if (!c || !st || !out_img || !out_depth || !v_output || !v_depth || !bg || !v_combined || !v_z) return BG_ERR_NULL;
-    if (((uintptr_t)out_depth | (uintptr_t)v_depth | (uintptr_t)v_z) % 4) {
-        set_err("bg_rasterize_backward_depth: out_depth, v_depth and v_z must be 4-byte aligned", cudaSuccess);
-        return BG_ERR_INVALID;
-    }
+    if (((uintptr_t)out_depth | (uintptr_t)v_depth | (uintptr_t)v_z) % 4)
+        return invalid("bg_rasterize_backward_depth", "out_depth, v_depth and v_z must be 4-byte aligned");
     return rasterize_backward(c, stream, st, out_img, out_depth, v_output, v_depth, bg, smooth, v_combined, rows, v_z,
                               "bg_rasterize_backward_depth");
 }
@@ -429,7 +375,7 @@ extern "C" int32_t bg_debug_blend_stats(BgContext *c, void *stream, const BgRend
                                         const float *v_output, const float *bg, float *v_combined_scratch,
                                         unsigned long long *out4) {
     if (!c || !st || !out_img || !v_output || !bg || !v_combined_scratch || !out4) return BG_ERR_NULL;
-    if (st->pass != BG_PASS_BACKWARD || st->tile_offsets != c->tile_offsets) { set_err("bg_debug_blend_stats: needs the state of this context's last Backward pass", cudaSuccess); return BG_ERR_INVALID; }
+    if (st->pass != BG_PASS_BACKWARD || st->tile_offsets != c->tile_offsets) return invalid("bg_debug_blend_stats", "needs the state of this context's last Backward pass");
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
     BG_CUDA(cudaMemsetAsync(c->blend_stats, 0, 4 * sizeof(unsigned long long), s));
@@ -448,15 +394,13 @@ extern "C" int32_t bg_project_backward(BgContext *c, void *stream, const BgCamer
                                        float *v_refine) {
     if (!c || !cam || !st || !v_combined || !v_transforms || !v_sh || !v_raw_opac || !v_refine) return BG_ERR_NULL;
     if (st->n > 0 && (!transforms || !sh || !raw_opac)) return BG_ERR_NULL;
-    const int deg = sh_degree_from_k(st->k);
-    if (deg < 0) return BG_ERR_INVALID;
+    int deg;
+    if (int32_t r = check_k(st->k, &deg); r != BG_OK) return r;
     if (cam->camera_model > BG_CAMERA_THIN_PRISM_FISHEYE) return BG_ERR_UNSUPPORTED;
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
-    if (((uintptr_t)sh | (uintptr_t)v_sh) % 16) {
-        set_err("bg_project_backward: sh and v_sh must be 16-byte aligned (128-bit row access)", cudaSuccess);
-        return BG_ERR_INVALID;
-    }
+    if (((uintptr_t)sh | (uintptr_t)v_sh) % 16)
+        return invalid("bg_project_backward", "sh and v_sh must be 16-byte aligned (128-bit row access)");
     BG_CUDA(launch_project_bwd(s, st->mip != 0, deg, transforms, sh, raw_opac, st->compact_from_global_gid, v_combined,
                                st->n, *cam, v_transforms, v_sh, v_raw_opac, v_refine, nullptr));
     return BG_OK;
@@ -467,7 +411,7 @@ extern "C" int32_t bg_project_backward_depth(BgContext *c, void *stream, const B
                                              const float *v_combined, const float *v_z, float *v_transforms, float *v_sh,
                                              float *v_raw_opac, float *v_refine) {
     if (!v_z) return BG_ERR_NULL;
-    if ((uintptr_t)v_z % 4) { set_err("bg_project_backward_depth: v_z must be 4-byte aligned", cudaSuccess); return BG_ERR_INVALID; }
+    if ((uintptr_t)v_z % 4) return invalid("bg_project_backward_depth", "v_z must be 4-byte aligned");
     const int32_t r = bg_project_backward(c, stream, cam, st, transforms, sh, raw_opac, v_combined, v_transforms, v_sh,
                                           v_raw_opac, v_refine);
     if (r != BG_OK) return r;
@@ -481,15 +425,13 @@ extern "C" int32_t bg_project_backward_factored(BgContext *c, void *stream, cons
                                                 float *v_raw_opac, float *v_refine) {
     if (!c || !cam || !st || !v_combined || !v_transforms || !v_color || !v_raw_opac || !v_refine) return BG_ERR_NULL;
     if (st->n > 0 && (!transforms || !sh || !raw_opac)) return BG_ERR_NULL;
-    const int deg = sh_degree_from_k(st->k);
-    if (deg < 0) return BG_ERR_INVALID;
+    int deg;
+    if (int32_t r = check_k(st->k, &deg); r != BG_OK) return r;
     if (cam->camera_model > BG_CAMERA_THIN_PRISM_FISHEYE) return BG_ERR_UNSUPPORTED;
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
-    if ((uintptr_t)sh % 16) {
-        set_err("bg_project_backward_factored: sh must be 16-byte aligned (128-bit row access)", cudaSuccess);
-        return BG_ERR_INVALID;
-    }
+    if ((uintptr_t)sh % 16)
+        return invalid("bg_project_backward_factored", "sh must be 16-byte aligned (128-bit row access)");
     BG_CUDA(launch_project_bwd(s, st->mip != 0, deg, transforms, sh, raw_opac, st->compact_from_global_gid, v_combined,
                                st->n, *cam, v_transforms, nullptr, v_raw_opac, v_refine, v_color));
     return BG_OK;
@@ -502,9 +444,9 @@ extern "C" int32_t bg_sh_grad_from_views(BgContext *c, void *stream, uint32_t n,
     if (n == 0) return BG_OK;
     if (!transforms || !cam_positions || !v_color_all || !v_sh) return BG_ERR_NULL;
     const int deg = sh_degree_from_k(k);
-    if (deg < 0 || views == 0 || views > 16) { set_err("bg_sh_grad_from_views: k must be a square <= 25, 1 <= views <= 16", cudaSuccess); return BG_ERR_INVALID; }
+    if (deg < 0 || views == 0 || views > 16) return invalid("bg_sh_grad_from_views", "k must be a square <= 25, 1 <= views <= 16");
     BG_CUDA(cudaSetDevice(c->device));
-    if (view_stride != 0 && view_stride < (uint64_t)n * 3) { set_err("bg_sh_grad_from_views: view_stride smaller than one view", cudaSuccess); return BG_ERR_INVALID; }
+    if (view_stride != 0 && view_stride < (uint64_t)n * 3) return invalid("bg_sh_grad_from_views", "view_stride smaller than one view");
     BG_CUDA(launch_sh_grad_from_views((cudaStream_t)stream, deg, transforms, v_color_all, n, cam_positions, views, out_scale, v_sh,
                                       view_stride ? (size_t)view_stride : (size_t)n * 3));
     return BG_OK;
@@ -517,7 +459,7 @@ extern "C" int32_t bg_radix_argsort_u32(BgContext *c, void *stream, const uint32
     if (n == 0) return BG_OK;
     if (!keys || !vals || !keys_out || !vals_out) return BG_ERR_NULL;
     if (bits > 32) { set_err("Can only sort up to 32 bits", cudaSuccess); return BG_ERR_INVALID; }
-    if (n > std::max(c->max_n, c->max_isect)) { set_err("bg_radix_argsort_u32: n exceeds context capacity", cudaSuccess); return BG_ERR_CAPACITY; }
+    if (n > sort_capacity(c)) return capacity("bg_radix_argsort_u32", "n exceeds context capacity");
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
     uint32_t *ctl2 = c->ctl + CTL_WORDS;
@@ -550,7 +492,7 @@ extern "C" int32_t bg_inclusive_scan_u32(BgContext *c, void *stream, const uint3
     if (!in || !out) return BG_ERR_NULL;
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
-    if ((uint64_t)(n + 2047) / 2048 > c->lb_scan_words) { set_err("bg_inclusive_scan_u32: n exceeds context capacity", cudaSuccess); return BG_ERR_CAPACITY; }
+    if ((uint64_t)(n + 2047) / 2048 > c->lb_scan_words) return capacity("bg_inclusive_scan_u32", "n exceeds context capacity");
     uint32_t *ctl2 = c->ctl + CTL_WORDS;
     BG_CUDA(launch_bump_epoch(s, c->epoch_dev));
     BG_CUDA(cudaMemsetAsync(ctl2 + CTL_TICKETS, 0, 48 * sizeof(uint32_t), s));
@@ -604,16 +546,12 @@ extern "C" int32_t bg_depth_loss_fused(BgContext *c, void *stream, const float *
                                        const float *target, uint32_t h, uint32_t w, float chain, float *v_output,
                                        float *v_depth, float *partials) {
     if (!c || !out_img || !depth || !target || !v_output || !v_depth || !partials) return BG_ERR_NULL;
-    if (h == 0 || w == 0) { set_err("bg_depth_loss_fused: empty image", cudaSuccess); return BG_ERR_INVALID; }
-    if (!(chain >= 0.0f) || !std::isfinite(chain)) { set_err("bg_depth_loss_fused: chain must be finite and >= 0", cudaSuccess); return BG_ERR_INVALID; }
-    if ((((uintptr_t)out_img) | ((uintptr_t)v_output)) & 15u) {
-        set_err("bg_depth_loss_fused: out_img and v_output must be 16-byte aligned (128-bit pixel access)", cudaSuccess);
-        return BG_ERR_INVALID;
-    }
-    if ((((uintptr_t)depth) | ((uintptr_t)target) | ((uintptr_t)v_depth) | ((uintptr_t)partials)) & 3u) {
-        set_err("bg_depth_loss_fused: depth, target, v_depth and partials must be 4-byte aligned", cudaSuccess);
-        return BG_ERR_INVALID;
-    }
+    if (h == 0 || w == 0) return invalid("bg_depth_loss_fused", "empty image");
+    if (!(chain >= 0.0f) || !std::isfinite(chain)) return invalid("bg_depth_loss_fused", "chain must be finite and >= 0");
+    if ((((uintptr_t)out_img) | ((uintptr_t)v_output)) & 15u)
+        return invalid("bg_depth_loss_fused", "out_img and v_output must be 16-byte aligned (128-bit pixel access)");
+    if ((((uintptr_t)depth) | ((uintptr_t)target) | ((uintptr_t)v_depth) | ((uintptr_t)partials)) & 3u)
+        return invalid("bg_depth_loss_fused", "depth, target, v_depth and partials must be 4-byte aligned");
     BG_CUDA(cudaSetDevice(c->device));
     BG_CUDA(launch_depth_loss_fused((cudaStream_t)stream, out_img, depth, target, h, w, chain, v_output, v_depth, partials));
     return BG_OK;
@@ -638,7 +576,7 @@ extern "C" int32_t bg_adam_step(BgContext *c, void *stream, float *p, const floa
     if (!c) return BG_ERR_NULL;
     if (rows == 0 || cols == 0) return BG_OK;
     if (!p || !g || !m || !v) return BG_ERR_NULL;
-    if (t < 1) { set_err("bg_adam_step: t is 1-based", cudaSuccess); return BG_ERR_INVALID; }
+    if (t < 1) return invalid("bg_adam_step", "t is 1-based");
     BG_CUDA(cudaSetDevice(c->device));
     const float bc1 = 1.0f - powi_f32(beta1, t), bc2 = 1.0f - powi_f32(beta2, t);
     BG_CUDA(launch_adam((cudaStream_t)stream, p, g, m, v, rows, cols, lr_scale, lr, beta1, beta2, eps, bc1, bc2, t == 1,
@@ -667,8 +605,8 @@ extern "C" int32_t bg_compute_min_scale(BgContext *c, void *stream, uint32_t n, 
     if (!c) return BG_ERR_NULL;
     if (n == 0) return BG_OK;
     if (!transforms || !view_cams || !f_out) return BG_ERR_NULL;
-    if (views == 0 || !(factor > 0.0f)) { set_err("bg_compute_min_scale: needs views > 0 and factor > 0 (the reference returns None)", cudaSuccess); return BG_ERR_INVALID; }
-    if ((uintptr_t)view_cams % 16) { set_err("bg_compute_min_scale: view_cams must be 16-byte aligned", cudaSuccess); return BG_ERR_INVALID; }
+    if (views == 0 || !(factor > 0.0f)) return invalid("bg_compute_min_scale", "needs views > 0 and factor > 0 (the reference returns None)");
+    if ((uintptr_t)view_cams % 16) return invalid("bg_compute_min_scale", "view_cams must be 16-byte aligned");
     BG_CUDA(cudaSetDevice(c->device));
     BG_CUDA(launch_min_scale((cudaStream_t)stream, n, transforms, view_cams, views, factor, f_out));
     return BG_OK;
@@ -745,14 +683,12 @@ extern "C" int32_t bg_train_update(BgContext *c, void *stream, const BgTrainUpda
         !a->refine_norm || !a->vis_weight || !a->max_screen || !a->v_transforms || !a->v_sh_grad || !a->v_raw_opac ||
         !a->v_refine || !a->visible || !a->max_radius)
         return BG_ERR_NULL;
-    const int deg = sh_degree_from_k(a->k);
-    if (deg < 0) { set_err("Invalid nr. of sh bases", cudaSuccess); return BG_ERR_INVALID; }
-    if (a->step < 1) { set_err("bg_train_update: step is 1-based", cudaSuccess); return BG_ERR_INVALID; }
-    if (!update_aligned(a) || (uintptr_t)a->v_transforms % 8 || (uintptr_t)a->v_sh_grad % 16) {
-        set_err("bg_train_update: transforms, m_t, v_t and v_transforms must be 8-byte aligned, sh, m_sh and v_sh_grad "
-                "16-byte aligned (64- and 128-bit row access)", cudaSuccess);
-        return BG_ERR_INVALID;
-    }
+    int deg;
+    if (int32_t r = check_k(a->k, &deg); r != BG_OK) return r;
+    if (a->step < 1) return invalid("bg_train_update", "step is 1-based");
+    if (!update_aligned(a) || (uintptr_t)a->v_transforms % 8 || (uintptr_t)a->v_sh_grad % 16)
+        return invalid("bg_train_update", "transforms, m_t, v_t and v_transforms must be 8-byte aligned, sh, m_sh and v_sh_grad "
+                                          "16-byte aligned (64- and 128-bit row access)");
     BG_CUDA(cudaSetDevice(c->device));
     UpdateParams P = update_params(a);
     P.g_t = a->v_transforms; P.g_o = a->v_raw_opac; P.g_sh = a->v_sh_grad;
@@ -777,6 +713,14 @@ struct Carver {
         return p;
     }
 };
+
+// the input and the output pair of one bg_radix_argsort_u32 over n keys; the base of the workspaces that sort
+struct SortWs {
+    uint32_t *keys, *vals, *keys_s, *vals_s;
+};
+void carve_sort_ws(Carver &cv, uint32_t n, SortWs &w) {
+    w.keys = cv.take<uint32_t>(n); w.vals = cv.take<uint32_t>(n); w.keys_s = cv.take<uint32_t>(n); w.vals_s = cv.take<uint32_t>(n);
+}
 
 struct TrainWs {
     float *out_img, *v_output, *partials, *v_combined, *v_t, *v_sh, *v_o, *v_r, *visible, *max_radius;
@@ -824,16 +768,10 @@ int32_t check_train_args(const A *a, const char *who) {
     if (!a->transforms || !a->sh || !a->raw_opac || !a->m_t || !a->v_t || !a->m_sh || !a->v_sh || !a->m_o || !a->v_o ||
         !a->refine_norm || !a->vis_weight || !a->max_screen || !a->gt_packed || !a->workspace || !a->loss_out)
         return BG_ERR_NULL;
-    char m[160];
-    auto invalid = [&](const char *what) {
-        snprintf(m, sizeof(m), "%s: %s", who, what);
-        set_err(m, cudaSuccess);
-        return BG_ERR_INVALID;
-    };
-    if (a->step < 1) return invalid("step is 1-based");
-    if (a->channels != 3 && a->channels != 4) return invalid("channels must be 3 or 4");
-    if ((uintptr_t)a->workspace % 256) return invalid("workspace must be 256-byte aligned");
-    if (!update_aligned(a)) return invalid("transforms, m_t and v_t must be 8-byte aligned, sh and m_sh 16-byte aligned");
+    if (a->step < 1) return invalid(who, "step is 1-based");
+    if (a->channels != 3 && a->channels != 4) return invalid(who, "channels must be 3 or 4");
+    if (int32_t r = check_workspace_aligned(who, a->workspace); r != BG_OK) return r;
+    if (!update_aligned(a)) return invalid(who, "transforms, m_t and v_t must be 8-byte aligned, sh and m_sh 16-byte aligned");
     return BG_OK;
 }
 
@@ -842,12 +780,7 @@ bool depth_term(const BgDepthSupervision &d) { return d.weight > 0.0f && d.valid
 
 int32_t check_depth(const BgDepthSupervision &d, const char *who) {
     if (!d.depth_loss_out) return BG_ERR_NULL;
-    if (!(d.weight >= 0.0f) || !std::isfinite(d.weight)) {
-        char m[160];
-        snprintf(m, sizeof(m), "%s: weight must be finite and >= 0", who);
-        set_err(m, cudaSuccess);
-        return BG_ERR_INVALID;
-    }
+    if (!(d.weight >= 0.0f) || !std::isfinite(d.weight)) return invalid(who, "weight must be finite and >= 0");
     if (depth_term(d) && !d.target) return BG_ERR_NULL;
     return BG_OK;
 }
@@ -886,16 +819,14 @@ extern "C" uint64_t bg_train_step_depth_workspace_bytes(uint32_t n, uint32_t k, 
 // The single-view step.  d == nullptr: bg_train_step.  Otherwise the step with the depth term of DESIGN.md section 4.7
 // (d validated, its term on, by bg_train_step_depth).
 static int32_t train_step(BgContext *c, void *stream, BgTrainStepArgs *a, const BgDepthSupervision *d) {
-    if (int32_t r = check_train_args(a, d ? "bg_train_step_depth" : "bg_train_step"); r != BG_OK) return r;
+    const char *who = d ? "bg_train_step_depth" : "bg_train_step";
+    if (int32_t r = check_train_args(a, who); r != BG_OK) return r;
     const uint32_t n = a->n, k = a->k, w = a->w, h = a->h;
     const TrainWs ws = carve_train_ws(a->workspace, n, k, w, h, a->channels);
     // the depth term's buffers; all null without the term, which selects the plain render and blend backward
     const DepthWs dws = carve_depth_ws(d ? a->workspace : nullptr, bg_train_step_workspace_bytes(n, k, w, h), n, w, h);
-    if ((d ? dws.bytes : ws.bytes) > a->workspace_bytes) {
-        set_err(d ? "bg_train_step_depth: workspace too small (bg_train_step_depth_workspace_bytes)"
-                  : "bg_train_step: workspace too small (bg_train_step_workspace_bytes)", cudaSuccess);
-        return BG_ERR_CAPACITY;
-    }
+    if (int32_t r = check_workspace_bytes(who, d ? "bg_train_step_depth_workspace_bytes" : "bg_train_step_workspace_bytes",
+                                          a->workspace_bytes, d ? dws.bytes : ws.bytes); r != BG_OK) return r;
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
     int32_t r;
@@ -961,7 +892,7 @@ extern "C" int32_t bg_dp_unique_id(uint8_t *out_id) {
 extern "C" int32_t bg_dp_comm_create(BgContext *c, const uint8_t *id_bytes, int32_t rank, int32_t world, BgDpComm **out) {
     if (!c || !id_bytes || !out) return BG_ERR_NULL;
     *out = nullptr;
-    if (world < 1 || rank < 0 || rank >= world) { set_err("bg_dp_comm_create: rank/world", cudaSuccess); return BG_ERR_INVALID; }
+    if (world < 1 || rank < 0 || rank >= world) return invalid("bg_dp_comm_create", "rank/world");
     NcclUniqueId id;
     memcpy(id.internal, id_bytes, BG_DP_UNIQUE_ID_BYTES);
     int rc = 0;
@@ -991,7 +922,7 @@ extern "C" int32_t bg_dp_pack_view(BgContext *c, void *stream, uint32_t n, uint3
     if (!c) return BG_ERR_NULL;
     if (n == 0) return BG_OK;
     if (!v_t || !v_o || !v_color || !v_refine || !visible || !max_radius || !small || !stat || !record) return BG_ERR_NULL;
-    if (local == 0 || local > DP_MAX_VIEWS || view >= local) { set_err("bg_dp_pack_view: view index / views per rank", cudaSuccess); return BG_ERR_INVALID; }
+    if (local == 0 || local > DP_MAX_VIEWS || view >= local) return invalid("bg_dp_pack_view", "view index / views per rank");
     BG_CUDA(cudaSetDevice(c->device));
     BG_CUDA(launch_pack_view((cudaStream_t)stream, n, local, view, first != 0, v_t, v_o, v_color, v_refine, visible, max_radius, small, stat, record));
     return BG_OK;
@@ -1017,10 +948,8 @@ extern "C" int32_t bg_dp_exchange(BgContext *c, BgDpComm *h, void *stream, uint3
                                   const float *record, float *recv, uint32_t chunks) {
     if (!c || !h || !small || !stat || !record || !recv) return BG_ERR_NULL;
     if (n == 0) return BG_OK;
-    if (local == 0 || local * (uint32_t)h->c->world > DP_MAX_VIEWS || chunks == 0 || chunks > DP_MAX_CHUNKS) {
-        set_err("bg_dp_exchange: 1..16 views in total, 1..16 chunks", cudaSuccess);
-        return BG_ERR_INVALID;
-    }
+    if (local == 0 || local * (uint32_t)h->c->world > DP_MAX_VIEWS || chunks == 0 || chunks > DP_MAX_CHUNKS)
+        return invalid("bg_dp_exchange", "1..16 views in total, 1..16 chunks");
     BG_CUDA(cudaSetDevice(c->device));
     cudaStream_t s = (cudaStream_t)stream;
     int32_t r = issue_exchange(h->c, s, n, local, chunks, small, stat, record, recv, nullptr, nullptr);
@@ -1060,10 +989,6 @@ ViewsWs carve_views_ws(void *base, uint32_t n, uint32_t w, uint32_t h, uint32_t 
     return ws;
 }
 }  // namespace
-
-namespace bg {
-cudaError_t launch_loss_mean(cudaStream_t, const float *, uint32_t, float *);
-}
 
 // BG_DP_TRACE=1: device timeline of the multi-device step (stderr, rank 0 only; synchronises -- a debugging aid)
 namespace {
@@ -1115,20 +1040,20 @@ static int32_t train_step_views(BgContext *c, BgDpComm *h, void *stream, BgTrain
     const uint32_t n = a->n, k = a->k, w = a->w, hh = a->h, local = a->local_views;
     const uint32_t world = h ? (uint32_t)h->c->world : 1u;
     const uint32_t views = local * world;
-    if (local == 0 || views > DP_MAX_VIEWS) { set_err("bg_train_step_views: 1..16 views per step in total", cudaSuccess); return BG_ERR_INVALID; }
-    const int deg = sh_degree_from_k(k);
-    if (deg < 0) { set_err("Invalid nr. of sh bases", cudaSuccess); return BG_ERR_INVALID; }
+    if (local == 0 || views > DP_MAX_VIEWS) return invalid("bg_train_step_views", "1..16 views per step in total");
+    int deg;
+    if (int32_t r = check_k(k, &deg); r != BG_OK) return r;
     for (uint32_t i = 0; i < local; i++)
         if (!a->gt_packed[i]) return BG_ERR_NULL;
     const bool fold = a->min_scale != nullptr;
     const ViewsWs ws = carve_views_ws(a->workspace, n, w, hh, local, world, fold);
-    if (ws.bytes > a->workspace_bytes) { set_err("bg_train_step_views: workspace too small (bg_train_step_views_workspace_bytes)", cudaSuccess); return BG_ERR_CAPACITY; }
-    if (a->chunks > DP_MAX_CHUNKS) { set_err("bg_train_step_views: at most 16 chunks", cudaSuccess); return BG_ERR_INVALID; }
+    if (int32_t r = check_workspace_bytes("bg_train_step_views", "bg_train_step_views_workspace_bytes", a->workspace_bytes, ws.bytes); r != BG_OK)
+        return r;
+    if (a->chunks > DP_MAX_CHUNKS) return invalid("bg_train_step_views", "at most 16 chunks");
     const DepthWs dws = carve_depth_ws(a->workspace, bg_train_step_views_workspace_bytes(n, k, w, hh, local, world), n, w, hh);
-    if (dep && dws.bytes > a->workspace_bytes) {
-        set_err("bg_train_step_views_depth: workspace too small (bg_train_step_views_depth_workspace_bytes)", cudaSuccess);
-        return BG_ERR_CAPACITY;
-    }
+    if (int32_t r = check_workspace_bytes("bg_train_step_views_depth", "bg_train_step_views_depth_workspace_bytes", a->workspace_bytes,
+                                          dep ? dws.bytes : 0); r != BG_OK)
+        return r;
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
     int32_t r;
@@ -1238,21 +1163,19 @@ extern "C" int32_t bg_train_step_views(BgContext *c, BgDpComm *h, void *stream, 
 extern "C" int32_t bg_train_step_views_depth(BgContext *c, BgDpComm *h, void *stream, BgTrainViewsArgs *a, const BgDepthSupervision *depth) {
     if (!c || !a || !depth) return BG_ERR_NULL;
     const uint32_t local = a->local_views;
-    if (local == 0 || local > DP_MAX_VIEWS) { set_err("bg_train_step_views_depth: 1..16 views per step in total", cudaSuccess); return BG_ERR_INVALID; }
+    if (local == 0 || local > DP_MAX_VIEWS) return invalid("bg_train_step_views_depth", "1..16 views per step in total");
     for (uint32_t i = 0; i < local; i++) {
         if (int32_t r = check_depth(depth[i], "bg_train_step_views_depth"); r != BG_OK) return r;
-        if (depth_term(depth[i]) && (uintptr_t)depth[i].target % 4) {
-            set_err("bg_train_step_views_depth: target must be 4-byte aligned", cudaSuccess);
-            return BG_ERR_INVALID;
-        }
+        if (depth_term(depth[i]) && (uintptr_t)depth[i].target % 4)
+            return invalid("bg_train_step_views_depth", "target must be 4-byte aligned");
     }
     return train_step_views(c, h, stream, a, depth);
 }
 
 // ---- refine (refine.cu): every decision on the device, one readback of the counts at the end
 namespace {
-struct RefineWs {
-    uint32_t *ctl, *keep, *keep_incl, *keys, *vals, *keys_s, *vals_s, *split, *cand, *cand_incl, *split_incl;
+struct RefineWs : SortWs {
+    uint32_t *ctl, *keep, *keep_incl, *split, *cand, *cand_incl, *split_incl;
     float *refine_norm, *vis_weight, *max_screen, *bounds_out;
     uint64_t bytes;
 };
@@ -1261,7 +1184,8 @@ RefineWs carve_refine_ws(void *base, uint32_t n) {
     auto take = [&](uint64_t words) { return cv.take<uint32_t>(words); };
     RefineWs w;
     w.ctl = take(64);
-    w.keep = take(n); w.keep_incl = take(n); w.keys = take(n); w.vals = take(n); w.keys_s = take(n); w.vals_s = take(n);
+    w.keep = take(n); w.keep_incl = take(n);
+    carve_sort_ws(cv, n, w);
     w.split = take(n); w.cand = take(n); w.cand_incl = take(n); w.split_incl = take(n);
     w.refine_norm = cv.take(n); w.vis_weight = cv.take(n); w.max_screen = cv.take(n);
     w.bounds_out = cv.take(16);
@@ -1281,12 +1205,12 @@ extern "C" int32_t bg_refine(BgContext *c, void *stream, const BgRefineArgs *a, 
         !a->refine_norm || !a->vis_weight || !a->max_screen || !a->transforms_out || !a->sh_out || !a->raw_opac_out ||
         !a->m_t_out || !a->v_t_out || !a->m_sh_out || !a->v_sh_out || !a->m_o_out || !a->v_o_out || !a->workspace)
         return BG_ERR_NULL;
-    if (sh_degree_from_k(a->k) < 0) { set_err("Invalid nr. of sh bases", cudaSuccess); return BG_ERR_INVALID; }
-    if (a->capacity < n0) { set_err("bg_refine: capacity smaller than n", cudaSuccess); return BG_ERR_CAPACITY; }
-    if ((uintptr_t)a->workspace % 256) { set_err("bg_refine: workspace must be 256-byte aligned", cudaSuccess); return BG_ERR_INVALID; }
+    int32_t r;
+    if ((r = check_k(a->k)) != BG_OK) return r;
+    if (a->capacity < n0) return capacity("bg_refine", "capacity smaller than n");
     const RefineWs w = carve_refine_ws(a->workspace, n0);
-    if (w.bytes > a->workspace_bytes) { set_err("bg_refine: workspace too small (bg_refine_workspace_bytes)", cudaSuccess); return BG_ERR_CAPACITY; }
-    if (n0 > std::max(c->max_n, c->max_isect)) { set_err("bg_refine: n exceeds the context's sort capacity", cudaSuccess); return BG_ERR_CAPACITY; }
+    if ((r = check_workspace("bg_refine", "bg_refine_workspace_bytes", a->workspace, a->workspace_bytes, w.bytes)) != BG_OK) return r;
+    if (n0 > sort_capacity(c)) return capacity("bg_refine", "n exceeds the context's sort capacity");
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
     const uint32_t kf = a->k * 3;
@@ -1296,7 +1220,6 @@ extern "C" int32_t bg_refine(BgContext *c, void *stream, const BgRefineArgs *a, 
     p.transforms_out = a->transforms_out; p.sh_out = a->sh_out; p.raw_opac_out = a->raw_opac_out; p.m_t_out = a->m_t_out;
     p.v_t_out = a->v_t_out; p.m_sh_out = a->m_sh_out; p.v_sh_out = a->v_sh_out; p.m_o_out = a->m_o_out; p.v_o_out = a->v_o_out;
     p.refine_norm_tmp = w.refine_norm; p.vis_weight_tmp = w.vis_weight; p.max_screen_tmp = w.max_screen;
-    int32_t r;
     BG_CUDA(cudaMemsetAsync(w.ctl, 0, 64 * sizeof(uint32_t), s));
     BG_CUDA(cudaMemsetAsync(w.split, 0, (size_t)n0 * sizeof(uint32_t), s));
     // prune mask -> flag scan -> compaction of all rows (train.rs:487-535, 848-893)
@@ -1332,7 +1255,7 @@ extern "C" int32_t bg_refine(BgContext *c, void *stream, const BgRefineArgs *a, 
     out->num_pruned = host[RC_PRUNED];
     out->num_pruned_non_finite = host[RC_NON_FINITE];
     out->total_splats = host[RC_N_NEW];
-    if (host[RC_OVERFLOW]) { set_err("bg_refine: capacity of the destination arrays exceeded", cudaSuccess); return BG_ERR_CAPACITY; }
+    if (host[RC_OVERFLOW]) return capacity("bg_refine", "capacity of the destination arrays exceeded");
     return BG_OK;
 }
 
@@ -1343,7 +1266,7 @@ extern "C" int32_t bg_bounds_percentile(BgContext *c, void *stream, uint32_t n, 
     if (n == 0) return BG_OK;
     if (!transforms || !workspace) return BG_ERR_NULL;
     const RefineWs w = carve_refine_ws(workspace, n);
-    if (w.bytes > workspace_bytes) { set_err("bg_bounds_percentile: workspace too small (bg_refine_workspace_bytes)", cudaSuccess); return BG_ERR_CAPACITY; }
+    if (int32_t r = check_workspace_bytes("bg_bounds_percentile", "bg_refine_workspace_bytes", workspace_bytes, w.bytes); r != BG_OK) return r;
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
     BG_CUDA(cudaMemsetAsync(w.ctl, 0, 64 * sizeof(uint32_t), s));
@@ -1378,21 +1301,12 @@ extern "C" int32_t bg_pup_log_det(BgContext *c, void *stream, uint32_t n, const 
     return BG_OK;
 }
 
-namespace {
-struct DecimateWs {
-    uint32_t *keys, *vals, *keys_s, *vals_s;
-    uint64_t bytes;
-};
-DecimateWs carve_decimate_ws(void *base, uint32_t n) {
-    Carver cv{base};
-    DecimateWs w;
-    w.keys = cv.take<uint32_t>(n); w.vals = cv.take<uint32_t>(n); w.keys_s = cv.take<uint32_t>(n); w.vals_s = cv.take<uint32_t>(n);
-    w.bytes = cv.off;
-    return w;
+extern "C" uint64_t bg_decimate_workspace_bytes(uint32_t n) {
+    Carver cv{nullptr};
+    SortWs w;
+    carve_sort_ws(cv, std::max(n, 1u), w);   // the sort's buffers are all of it
+    return cv.off;
 }
-}  // namespace
-
-extern "C" uint64_t bg_decimate_workspace_bytes(uint32_t n) { return carve_decimate_ws(nullptr, std::max(n, 1u)).bytes; }
 
 extern "C" int32_t bg_decimate_to_count(BgContext *c, void *stream, const BgDecimateArgs *a) {
     if (!c || !a) return BG_ERR_NULL;
@@ -1401,20 +1315,21 @@ extern "C" int32_t bg_decimate_to_count(BgContext *c, void *stream, const BgDeci
     if (!a->scores || !a->transforms || !a->sh || !a->raw_opac || !a->transforms_out || !a->sh_out || !a->raw_opac_out ||
         !a->workspace || (a->min_scale && !a->min_scale_out))
         return BG_ERR_NULL;
-    if (sh_degree_from_k(a->k) < 0) { set_err("Invalid nr. of sh bases", cudaSuccess); return BG_ERR_INVALID; }
+    int32_t r;
+    if ((r = check_k(a->k)) != BG_OK) return r;
     const void *ptrs[] = {a->transforms, a->sh, a->raw_opac, a->min_scale, a->transforms_out, a->sh_out, a->raw_opac_out,
                           a->min_scale_out, a->workspace};
     for (const void *p : ptrs)
-        if ((uintptr_t)p % 16) { set_err("bg_decimate_to_count: arrays must be 16-byte aligned", cudaSuccess); return BG_ERR_INVALID; }
-    if ((uintptr_t)a->workspace % 256) { set_err("bg_decimate_to_count: workspace must be 256-byte aligned", cudaSuccess); return BG_ERR_INVALID; }
-    const DecimateWs w = carve_decimate_ws(a->workspace, n);
-    if (w.bytes > a->workspace_bytes) { set_err("bg_decimate_to_count: workspace too small (bg_decimate_workspace_bytes)", cudaSuccess); return BG_ERR_CAPACITY; }
-    if (n > std::max(c->max_n, c->max_isect)) { set_err("bg_decimate_to_count: n exceeds the context's sort capacity", cudaSuccess); return BG_ERR_CAPACITY; }
+        if ((uintptr_t)p % 16) return invalid("bg_decimate_to_count", "arrays must be 16-byte aligned");
+    Carver cv{a->workspace};
+    SortWs w;
+    carve_sort_ws(cv, n, w);
+    if ((r = check_workspace("bg_decimate_to_count", "bg_decimate_workspace_bytes", a->workspace, a->workspace_bytes, cv.off)) != BG_OK) return r;
+    if (n > sort_capacity(c)) return capacity("bg_decimate_to_count", "n exceeds the context's sort capacity");
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
     BG_CUDA(launch_decimate_keys(s, n, a->scores, w.keys, w.vals));
-    int32_t r = bg_radix_argsort_u32(c, stream, w.keys, w.vals, n, nullptr, 32, w.keys_s, w.vals_s);
-    if (r != BG_OK) return r;
+    if ((r = bg_radix_argsort_u32(c, stream, w.keys, w.vals, n, nullptr, 32, w.keys_s, w.vals_s)) != BG_OK) return r;
     BG_CUDA(launch_decimate_gather(s, target, a->k * 3, w.vals_s, a->transforms, a->sh, a->raw_opac, a->min_scale,
                                    a->transforms_out, a->sh_out, a->raw_opac_out, a->min_scale_out));
     if (a->kept_ids_out) BG_CUDA(cudaMemcpyAsync(a->kept_ids_out, w.vals_s, (size_t)target * 4, cudaMemcpyDeviceToDevice, s));
@@ -1423,15 +1338,15 @@ extern "C" int32_t bg_decimate_to_count(BgContext *c, void *stream, const BgDeci
 
 // ---- Compressed PLY encoding (compress.cu, DESIGN.md section 4.8)
 namespace {
-struct CompressWs {
-    uint32_t *bounds, *keys, *vals, *keys_s, *vals_s;
+struct CompressWs : SortWs {
+    uint32_t *bounds;
     uint64_t bytes;
 };
 CompressWs carve_compress_ws(void *base, uint32_t n) {
     Carver cv{base};
     CompressWs w;
     w.bounds = cv.take<uint32_t>(8);
-    w.keys = cv.take<uint32_t>(n); w.vals = cv.take<uint32_t>(n); w.keys_s = cv.take<uint32_t>(n); w.vals_s = cv.take<uint32_t>(n);
+    carve_sort_ws(cv, n, w);
     w.bytes = cv.off;
     return w;
 }
@@ -1443,8 +1358,9 @@ extern "C" int32_t bg_compress_splats(BgContext *c, void *stream, const BgCompre
     if (!c || !a) return BG_ERR_NULL;
     const uint32_t n = a->n, k = a->k;
     if (!a->count_out) return BG_ERR_NULL;
-    if (sh_degree_from_k(k) < 0) { set_err("Invalid nr. of sh bases", cudaSuccess); return BG_ERR_INVALID; }
-    if ((uintptr_t)a->count_out % 4) { set_err("bg_compress_splats: count_out must be 4-byte aligned", cudaSuccess); return BG_ERR_INVALID; }
+    int32_t r;
+    if ((r = check_k(k)) != BG_OK) return r;
+    if ((uintptr_t)a->count_out % 4) return invalid("bg_compress_splats", "count_out must be 4-byte aligned");
     cudaStream_t s = (cudaStream_t)stream;
     if (n == 0) {
         BG_CUDA(cudaSetDevice(c->device));
@@ -1453,21 +1369,17 @@ extern "C" int32_t bg_compress_splats(BgContext *c, void *stream, const BgCompre
     }
     if (!a->transforms || !a->sh || !a->raw_opac || !a->chunks_out || !a->packed_out || !a->workspace || (k > 1 && !a->sh_out))
         return BG_ERR_NULL;
-    if (k == 1 && a->sh_out) { set_err("bg_compress_splats: sh_out must be NULL when k == 1", cudaSuccess); return BG_ERR_INVALID; }
+    if (k == 1 && a->sh_out) return invalid("bg_compress_splats", "sh_out must be NULL when k == 1");
     if (((uintptr_t)a->transforms | (uintptr_t)a->packed_out) % 16 ||
-        ((uintptr_t)a->sh | (uintptr_t)a->raw_opac | (uintptr_t)a->chunks_out | (uintptr_t)a->order_out) % 4) {
-        set_err("bg_compress_splats: transforms and packed_out must be 16-byte aligned, the other arrays 4-byte", cudaSuccess);
-        return BG_ERR_INVALID;
-    }
-    if ((uintptr_t)a->workspace % 256) { set_err("bg_compress_splats: workspace must be 256-byte aligned", cudaSuccess); return BG_ERR_INVALID; }
+        ((uintptr_t)a->sh | (uintptr_t)a->raw_opac | (uintptr_t)a->chunks_out | (uintptr_t)a->order_out) % 4)
+        return invalid("bg_compress_splats", "transforms and packed_out must be 16-byte aligned, the other arrays 4-byte");
     const CompressWs w = carve_compress_ws(a->workspace, n);
-    if (w.bytes > a->workspace_bytes) { set_err("bg_compress_splats: workspace too small (bg_compress_workspace_bytes)", cudaSuccess); return BG_ERR_CAPACITY; }
-    if (n > std::max(c->max_n, c->max_isect)) { set_err("bg_compress_splats: n exceeds the context's sort capacity", cudaSuccess); return BG_ERR_CAPACITY; }
+    if ((r = check_workspace("bg_compress_splats", "bg_compress_workspace_bytes", a->workspace, a->workspace_bytes, w.bytes)) != BG_OK) return r;
+    if (n > sort_capacity(c)) return capacity("bg_compress_splats", "n exceeds the context's sort capacity");
     BG_CUDA(cudaSetDevice(c->device));
     BG_CUDA(launch_compress_valid_bounds(s, n, k * 3, a->transforms, a->sh, a->raw_opac, w.keys, w.bounds));
     BG_CUDA(launch_compress_keys(s, n, a->transforms, w.bounds, w.keys, w.vals));
-    int32_t r = bg_radix_argsort_u32(c, stream, w.keys, w.vals, n, nullptr, 31, w.keys_s, w.vals_s);
-    if (r != BG_OK) return r;
+    if ((r = bg_radix_argsort_u32(c, stream, w.keys, w.vals, n, nullptr, 31, w.keys_s, w.vals_s)) != BG_OK) return r;
     BG_CUDA(launch_compress_chunks(s, n, k, a->transforms, a->sh, a->raw_opac, w.bounds, w.vals_s, a->chunks_out, a->packed_out,
                                    a->sh_out, a->order_out, a->count_out));
     return BG_OK;
@@ -1495,15 +1407,13 @@ MeshWs carve_mesh_ws(void *base, const uint32_t *dims) {
 }
 // Grid checks shared by the three calls: BG_OK, or the status with the message set.
 int32_t check_grid(const BgTsdfGrid *g, const char *who) {
-    char m[160];
     if (!g->tsdf || !g->weight || !g->rgb) return BG_ERR_NULL;
     const uint64_t np = (uint64_t)g->dims[0] * g->dims[1] * g->dims[2];
-    if (np == 0 || np >= (1ull << 31)) { snprintf(m, sizeof(m), "%s: grid dims must be non-zero with dx*dy*dz < 2^31", who); set_err(m, cudaSuccess); return BG_ERR_INVALID; }
-    if (((uintptr_t)g->tsdf | (uintptr_t)g->weight | (uintptr_t)g->rgb) % 4) { snprintf(m, sizeof(m), "%s: grid arrays must be 4-byte aligned", who); set_err(m, cudaSuccess); return BG_ERR_INVALID; }
+    if (np == 0 || np >= (1ull << 31)) return invalid(who, "grid dims must be non-zero with dx*dy*dz < 2^31");
+    if (((uintptr_t)g->tsdf | (uintptr_t)g->weight | (uintptr_t)g->rgb) % 4) return invalid(who, "grid arrays must be 4-byte aligned");
     if (!(g->h > 0.0f) || !std::isfinite(g->h) || !(g->trunc > 0.0f) || !std::isfinite(g->trunc) || !std::isfinite(g->origin[0]) ||
-        !std::isfinite(g->origin[1]) || !std::isfinite(g->origin[2])) {
-        snprintf(m, sizeof(m), "%s: grid origin must be finite, h and trunc finite and > 0", who); set_err(m, cudaSuccess); return BG_ERR_INVALID;
-    }
+        !std::isfinite(g->origin[1]) || !std::isfinite(g->origin[2]))
+        return invalid(who, "grid origin must be finite, h and trunc finite and > 0");
     return BG_OK;
 }
 }  // namespace
@@ -1513,13 +1423,11 @@ extern "C" int32_t bg_tsdf_integrate(BgContext *c, void *stream, const BgTsdfGri
     if (!c || !g || !cam || !out_img || !out_depth) return BG_ERR_NULL;
     int32_t r = check_grid(g, "bg_tsdf_integrate");
     if (r != BG_OK) return r;
-    if (w == 0 || h == 0) { set_err("bg_tsdf_integrate: empty image", cudaSuccess); return BG_ERR_INVALID; }
-    if (!(alpha_min > 0.0f && alpha_min <= 1.0f)) { set_err("bg_tsdf_integrate: alpha_min must be in (0, 1]", cudaSuccess); return BG_ERR_INVALID; }
-    if (cam->camera_model > BG_CAMERA_THIN_PRISM_FISHEYE) { set_err("bg_tsdf_integrate: unknown camera model", cudaSuccess); return BG_ERR_INVALID; }
-    if ((uintptr_t)out_img % 16 || (uintptr_t)out_depth % 4) {
-        set_err("bg_tsdf_integrate: out_img must be 16-byte aligned, out_depth 4-byte", cudaSuccess);
-        return BG_ERR_INVALID;
-    }
+    if (w == 0 || h == 0) return invalid("bg_tsdf_integrate", "empty image");
+    if (!(alpha_min > 0.0f && alpha_min <= 1.0f)) return invalid("bg_tsdf_integrate", "alpha_min must be in (0, 1]");
+    if (cam->camera_model > BG_CAMERA_THIN_PRISM_FISHEYE) return invalid("bg_tsdf_integrate", "unknown camera model");
+    if ((uintptr_t)out_img % 16 || (uintptr_t)out_depth % 4)
+        return invalid("bg_tsdf_integrate", "out_img must be 16-byte aligned, out_depth 4-byte");
     BG_CUDA(cudaSetDevice(c->device));
     BG_CUDA(launch_tsdf_integrate((cudaStream_t)stream, *g, *cam, w, h, out_img, out_depth, alpha_min));
     return BG_OK;
@@ -1530,17 +1438,6 @@ extern "C" uint64_t bg_mesh_workspace_bytes(uint32_t dx, uint32_t dy, uint32_t d
     return carve_mesh_ws(nullptr, dims).bytes;
 }
 
-namespace {
-int32_t mesh_ws_for(const BgTsdfGrid *g, void *ws, uint64_t ws_bytes, const char *who, MeshWs &w) {
-    char m[160];
-    if (!ws) return BG_ERR_NULL;
-    if ((uintptr_t)ws % 256) { snprintf(m, sizeof(m), "%s: workspace must be 256-byte aligned", who); set_err(m, cudaSuccess); return BG_ERR_INVALID; }
-    w = carve_mesh_ws(ws, g->dims);
-    if (w.bytes > ws_bytes) { snprintf(m, sizeof(m), "%s: workspace too small (bg_mesh_workspace_bytes)", who); set_err(m, cudaSuccess); return BG_ERR_CAPACITY; }
-    return BG_OK;
-}
-}  // namespace
-
 extern "C" int32_t bg_mesh_count(BgContext *c, void *stream, const BgTsdfGrid *g, void *ws, uint64_t ws_bytes, uint32_t *num_vertices,
                                  uint32_t *num_triangles) {
     if (!c || !g || !num_vertices || !num_triangles) return BG_ERR_NULL;
@@ -1548,15 +1445,15 @@ extern "C" int32_t bg_mesh_count(BgContext *c, void *stream, const BgTsdfGrid *g
     *num_triangles = 0;
     int32_t r = check_grid(g, "bg_mesh_count");
     if (r != BG_OK) return r;
-    MeshWs w;
-    if ((r = mesh_ws_for(g, ws, ws_bytes, "bg_mesh_count", w)) != BG_OK) return r;
+    const MeshWs w = carve_mesh_ws(ws, g->dims);
+    if ((r = check_workspace("bg_mesh_count", "bg_mesh_workspace_bytes", ws, ws_bytes, w.bytes)) != BG_OK) return r;
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
     BG_CUDA(launch_mesh_count(s, *g, w.brick_v, w.brick_t, w.voff, w.toff, w.header));
     unsigned long long host[2];
     BG_CUDA(cudaMemcpyAsync(host, w.header, sizeof(host), cudaMemcpyDeviceToHost, s));
     BG_CUDA(cudaStreamSynchronize(s));
-    if (host[0] > 0xFFFFFFFFull || host[1] > 0xFFFFFFFFull) { set_err("bg_mesh_count: more than 2^32 - 1 vertices or triangles", cudaSuccess); return BG_ERR_CAPACITY; }
+    if (host[0] > 0xFFFFFFFFull || host[1] > 0xFFFFFFFFull) return capacity("bg_mesh_count", "more than 2^32 - 1 vertices or triangles");
     *num_vertices = (uint32_t)host[0];
     *num_triangles = (uint32_t)host[1];
     return BG_OK;
@@ -1568,19 +1465,17 @@ extern "C" int32_t bg_mesh_emit(BgContext *c, void *stream, const BgTsdfGrid *g,
     int32_t r = check_grid(g, "bg_mesh_emit");
     if (r != BG_OK) return r;
     if ((max_vertices && (!vertices || !colors)) || (max_triangles && !faces)) return BG_ERR_NULL;
-    if (((uintptr_t)vertices | (uintptr_t)faces) % 4) { set_err("bg_mesh_emit: vertices and faces must be 4-byte aligned", cudaSuccess); return BG_ERR_INVALID; }
-    MeshWs w;
-    if ((r = mesh_ws_for(g, ws, ws_bytes, "bg_mesh_emit", w)) != BG_OK) return r;
+    if (((uintptr_t)vertices | (uintptr_t)faces) % 4) return invalid("bg_mesh_emit", "vertices and faces must be 4-byte aligned");
+    const MeshWs w = carve_mesh_ws(ws, g->dims);
+    if ((r = check_workspace("bg_mesh_emit", "bg_mesh_workspace_bytes", ws, ws_bytes, w.bytes)) != BG_OK) return r;
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
     unsigned long long host[5];
     BG_CUDA(cudaMemcpyAsync(host, w.header, sizeof(host), cudaMemcpyDeviceToHost, s));
     BG_CUDA(cudaStreamSynchronize(s));
-    if (host[2] != g->dims[0] || host[3] != g->dims[1] || host[4] != g->dims[2]) {
-        set_err("bg_mesh_emit: the workspace holds no bg_mesh_count of a grid with these dims", cudaSuccess);
-        return BG_ERR_INVALID;
-    }
-    if (host[0] > max_vertices || host[1] > max_triangles) { set_err("bg_mesh_emit: the mesh exceeds max_vertices / max_triangles", cudaSuccess); return BG_ERR_CAPACITY; }
+    if (host[2] != g->dims[0] || host[3] != g->dims[1] || host[4] != g->dims[2])
+        return invalid("bg_mesh_emit", "the workspace holds no bg_mesh_count of a grid with these dims");
+    if (host[0] > max_vertices || host[1] > max_triangles) return capacity("bg_mesh_emit", "the mesh exceeds max_vertices / max_triangles");
     if (host[0] == 0) return BG_OK;   // no vertices, so no triangles
     BG_CUDA(launch_mesh_emit(s, *g, w.voff, w.toff, w.vbase, w.vmask, max_vertices, max_triangles, vertices, colors, faces));
     return BG_OK;

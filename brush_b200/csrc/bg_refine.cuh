@@ -30,20 +30,34 @@ struct RefinePtrs {
     float *refine_norm_tmp, *vis_weight_tmp, *max_screen_tmp;
 };
 
-cudaError_t launch_refine_classify(cudaStream_t, uint32_t, uint32_t, const float *, const float *, const float *, const float *, float,
-                                   uint32_t *, uint32_t *);
-cudaError_t launch_refine_plan_prune(cudaStream_t, uint32_t, const uint32_t *, uint32_t *);
-cudaError_t launch_refine_compact(cudaStream_t, uint32_t, uint32_t, const RefinePtrs &, const uint32_t *, const uint32_t *, const uint32_t *);
-cudaError_t launch_refine_keys(cudaStream_t, uint32_t, int, const RefinePtrs &, float, uint64_t, uint64_t, uint32_t *, uint32_t *, uint32_t *);
-cudaError_t launch_refine_plan_growth(cudaStream_t, float, uint32_t, bool, uint32_t *);
-cudaError_t launch_refine_mark_topk(cudaStream_t, uint32_t, const uint32_t *, uint32_t, uint32_t, uint32_t, uint32_t *, uint32_t *);
-cudaError_t launch_refine_oversize_flags(cudaStream_t, uint32_t, float, const RefinePtrs &, const uint32_t *, uint32_t *, const uint32_t *);
-cudaError_t launch_refine_oversize_mark(cudaStream_t, uint32_t, uint32_t, const uint32_t *, const uint32_t *, uint32_t *, uint32_t *);
-cudaError_t launch_refine_plan_split(cudaStream_t, uint32_t, const uint32_t *, uint32_t, uint32_t *);
-cudaError_t launch_refine_split(cudaStream_t, uint32_t, uint32_t, uint32_t, float, const RefinePtrs &, const uint32_t *, const uint32_t *,
-                                const uint32_t *);
-cudaError_t launch_refine_decay(cudaStream_t, uint32_t, float, float *, const uint32_t *);
-cudaError_t launch_bounds_keys(cudaStream_t, uint32_t, int, const float *, uint32_t *, uint32_t *, uint32_t *);
-cudaError_t launch_bounds_pick(cudaStream_t, const uint32_t *, const uint32_t *, float, float *);
+// The launchers of refine.cu, in the order bg_refine issues them.  n0: splats before the prune; n_max = n0 bounds every
+// later pass, whose live count is ctl[RC_N] on the device.  kf = 3k floats per SH row.  ctl: the RC_* words above.
+// keep / split / cand [n0]: 0/1 flags; *_incl: their inclusive scans.
+// center: host [3]
+cudaError_t launch_refine_classify(cudaStream_t s, uint32_t n0, uint32_t kf, const float *transforms, const float *sh,
+                                   const float *raw_opac, const float *center, float max_allowed, uint32_t *keep, uint32_t *ctl);
+cudaError_t launch_refine_plan_prune(cudaStream_t s, uint32_t n0, const uint32_t *keep_incl, uint32_t *ctl);
+// the kept rows of every array of p -> its _out / _tmp arrays
+cudaError_t launch_refine_compact(cudaStream_t s, uint32_t n0, uint32_t kf, const RefinePtrs &p, const uint32_t *keep,
+                                  const uint32_t *keep_incl, const uint32_t *ctl);
+// sampling keys for the radix sort, vals = index.  mode 0: replacement of the pruned splats, 1: growth above grad_threshold
+cudaError_t launch_refine_keys(cudaStream_t s, uint32_t n_max, int mode, const RefinePtrs &p, float grad_threshold, uint64_t seed,
+                               uint64_t stream_id, uint32_t *keys, uint32_t *vals, uint32_t *ctl);
+cudaError_t launch_refine_plan_growth(cudaStream_t s, float fraction, uint32_t max_splats, bool enabled, uint32_t *ctl);
+// marks in split the first min(ctl[k_slot], ctl[pos_slot]) of sorted_vals; counts the new marks in ctl[count_slot]
+cudaError_t launch_refine_mark_topk(cudaStream_t s, uint32_t n_max, const uint32_t *sorted_vals, uint32_t k_slot, uint32_t pos_slot,
+                                    uint32_t count_slot, uint32_t *split, uint32_t *ctl);
+cudaError_t launch_refine_oversize_flags(cudaStream_t s, uint32_t n_max, float thr, const RefinePtrs &p, const uint32_t *split,
+                                         uint32_t *cand, const uint32_t *ctl);
+cudaError_t launch_refine_oversize_mark(cudaStream_t s, uint32_t n_max, uint32_t max_splats, const uint32_t *cand, const uint32_t *cand_incl,
+                                        uint32_t *split, uint32_t *ctl);
+cudaError_t launch_refine_plan_split(cudaStream_t s, uint32_t n_max, const uint32_t *split_incl, uint32_t capacity, uint32_t *ctl);
+cudaError_t launch_refine_split(cudaStream_t s, uint32_t n_max, uint32_t kf, uint32_t capacity, float thr, const RefinePtrs &p,
+                                const uint32_t *split, const uint32_t *split_incl, const uint32_t *ctl);
+cudaError_t launch_refine_decay(cudaStream_t s, uint32_t cap, float minus_opac, float *raw_opac, const uint32_t *ctl);
+// bg_bounds_percentile: keys = ordered bits of coordinate `axis` (non-finite ones last), *count += the finite ones;
+// out2 = the lower and upper bound that hold the central `percentile` of the first *count sorted_keys
+cudaError_t launch_bounds_keys(cudaStream_t s, uint32_t n, int axis, const float *transforms, uint32_t *keys, uint32_t *vals, uint32_t *count);
+cudaError_t launch_bounds_pick(cudaStream_t s, const uint32_t *sorted_keys, const uint32_t *count, float percentile, float *out2);
 
 }  // namespace bg

@@ -29,6 +29,7 @@
 // goes to the compact-indexed v_z[] (its factor, -1, sits in pad entry 10 of the factor row).  12 slots (slot 11 is
 // padding) cost one more shuffle in the first stage of the reduce-scatter.
 #include "blend_common.cuh"
+#include "bg_launch.cuh"
 
 namespace bg {
 

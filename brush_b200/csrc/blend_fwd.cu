@@ -14,6 +14,7 @@
 // 3 broadcast LDS.128, 4 scalar + 9 paired (18 scalar) FMA-pipe operations, 2 MUFU.EX2 and the pair tests.  The rows of a
 // batch are staged by TMA (per-row bulk copies, blend_common.cuh) into the warp's double buffer.
 #include "blend_common.cuh"
+#include "bg_launch.cuh"
 
 namespace bg {
 

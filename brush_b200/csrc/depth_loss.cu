@@ -14,6 +14,7 @@
 #include <algorithm>
 
 #include "bg_common.cuh"
+#include "bg_launch.cuh"
 
 namespace bg {
 

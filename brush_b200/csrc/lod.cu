@@ -12,6 +12,7 @@
 
 #include "bg_common.cuh"
 #include "bg_math.cuh"
+#include "bg_launch.cuh"
 
 namespace bg {
 

@@ -11,6 +11,7 @@
 // window sums follows the reference (symmetric pairs d=1..5, then the centre tap).
 // HBM-bound: ~28 P bytes forward, ~40 P backward for C=3.
 #include "bg_common.cuh"
+#include "bg_launch.cuh"
 
 namespace bg {
 

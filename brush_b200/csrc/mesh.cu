@@ -17,6 +17,7 @@
 #include "bg_common.cuh"
 #include "bg_math.cuh"
 #include "bg_project.cuh"
+#include "bg_launch.cuh"
 
 namespace bg {
 

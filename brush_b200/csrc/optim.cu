@@ -14,6 +14,7 @@
 #include "bg_common.cuh"
 #include "bg_fold.cuh"
 #include "bg_rng.cuh"
+#include "bg_launch.cuh"
 
 namespace bg {
 

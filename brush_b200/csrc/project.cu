@@ -17,6 +17,7 @@
 //     double buffered; the SH rows are read in index order there too, and the depth-ordered pass gathers one
 //     64-byte staged row per splat (two whole 32-byte sectors).
 #include "bg_project.cuh"
+#include "bg_launch.cuh"
 
 namespace bg {
 

@@ -11,6 +11,7 @@
 // gathered.  HBM-bound: (88+12K) V + (48+12K) N bytes (SURVEY.md 8d).
 #include "bg_project.cuh"
 #include "bg_sh.cuh"
+#include "bg_launch.cuh"
 
 namespace bg {
 

@@ -14,6 +14,7 @@
 // The element count may live on the device (n_dev): CTAs are persistent and pull tiles from a
 // ticket, so no host readback is needed to size the grid.
 #include "bg_common.cuh"
+#include "bg_launch.cuh"
 
 namespace bg {
 
