@@ -172,6 +172,17 @@ class BgTsdfGrid(C.Structure):
     ]
 
 
+class BgSparseTsdfGrid(C.Structure):
+    _fields_ = [
+        ("origin", C.c_float * 3), ("h", C.c_float),
+        ("dims", C.c_uint32 * 3), ("trunc", C.c_float),
+        ("brick_slot", C.c_void_p),
+        ("workspace", C.c_void_p), ("workspace_bytes", C.c_uint64),
+        ("num_bricks", C.c_uint32),
+        ("tsdf", C.c_void_p), ("weight", C.c_void_p), ("rgb", C.c_void_p),
+    ]
+
+
 class BgTrainViewsArgs(C.Structure):
     _fields_ = [
         ("w", C.c_uint32), ("h", C.c_uint32), ("n", C.c_uint32), ("k", C.c_uint32),
@@ -267,6 +278,13 @@ SIGNATURES = {
     "bg_mesh_workspace_bytes": (_U64, [_U32, _U32, _U32]),
     "bg_mesh_count": (_I32, [_P, _P, C.POINTER(BgTsdfGrid), _P, _U64, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
     "bg_mesh_emit": (_I32, [_P, _P, C.POINTER(BgTsdfGrid), _P, _U64, _U32, _U32, _P, _P, _P]),
+    "bg_sparse_tsdf_workspace_bytes": (_U64, [_U32, _U32, _U32, _U32, _U32]),
+    "bg_sparse_tsdf_mark": (_I32, [_P, _P, C.POINTER(BgSparseTsdfGrid), C.POINTER(BgCamera), _U32, _U32, _P, _P, C.c_float]),
+    "bg_sparse_tsdf_allocate": (_I32, [_P, _P, C.POINTER(BgSparseTsdfGrid), C.POINTER(C.c_uint32)]),
+    "bg_sparse_tsdf_integrate": (_I32, [_P, _P, C.POINTER(BgSparseTsdfGrid), C.POINTER(BgCamera), _U32, _U32, _P, _P, C.c_float]),
+    "bg_sparse_mesh_workspace_bytes": (_U64, [_U32]),
+    "bg_sparse_mesh_count": (_I32, [_P, _P, C.POINTER(BgSparseTsdfGrid), _P, _U64, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
+    "bg_sparse_mesh_emit": (_I32, [_P, _P, C.POINTER(BgSparseTsdfGrid), _P, _U64, _U32, _U32, _P, _P, _P]),
 }
 
 _lib = None

@@ -37,6 +37,7 @@ SOURCES = {
     "depth_loss.cu": ["-fmad=false"],
     "compress.cu": ["-fmad=false"],
     "mesh.cu": ["-fmad=false"],
+    "mesh_sparse.cu": ["-fmad=false"],
 }
 
 

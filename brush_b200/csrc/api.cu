@@ -1405,15 +1405,28 @@ MeshWs carve_mesh_ws(void *base, const uint32_t *dims) {
     w.bytes = cv.off;
     return w;
 }
+// Lattice checks shared by the dense and the sparse grid.
+int32_t check_lattice(const float *origin, float h, float trunc, const char *who) {
+    if (!(h > 0.0f) || !std::isfinite(h) || !(trunc > 0.0f) || !std::isfinite(trunc) || !std::isfinite(origin[0]) ||
+        !std::isfinite(origin[1]) || !std::isfinite(origin[2]))
+        return invalid(who, "grid origin must be finite, h and trunc finite and > 0");
+    return BG_OK;
+}
 // Grid checks shared by the three calls: BG_OK, or the status with the message set.
 int32_t check_grid(const BgTsdfGrid *g, const char *who) {
     if (!g->tsdf || !g->weight || !g->rgb) return BG_ERR_NULL;
     const uint64_t np = (uint64_t)g->dims[0] * g->dims[1] * g->dims[2];
     if (np == 0 || np >= (1ull << 31)) return invalid(who, "grid dims must be non-zero with dx*dy*dz < 2^31");
     if (((uintptr_t)g->tsdf | (uintptr_t)g->weight | (uintptr_t)g->rgb) % 4) return invalid(who, "grid arrays must be 4-byte aligned");
-    if (!(g->h > 0.0f) || !std::isfinite(g->h) || !(g->trunc > 0.0f) || !std::isfinite(g->trunc) || !std::isfinite(g->origin[0]) ||
-        !std::isfinite(g->origin[1]) || !std::isfinite(g->origin[2]))
-        return invalid(who, "grid origin must be finite, h and trunc finite and > 0");
+    return check_lattice(g->origin, g->h, g->trunc, who);
+}
+// One view's render and camera, as the integration and the marking take them.
+int32_t check_view(const BgCamera *cam, uint32_t w, uint32_t h, const float *out_img, const float *out_depth, float alpha_min,
+                   const char *who) {
+    if (w == 0 || h == 0) return invalid(who, "empty image");
+    if (!(alpha_min > 0.0f && alpha_min <= 1.0f)) return invalid(who, "alpha_min must be in (0, 1]");
+    if (cam->camera_model > BG_CAMERA_THIN_PRISM_FISHEYE) return invalid(who, "unknown camera model");
+    if ((uintptr_t)out_img % 16 || (uintptr_t)out_depth % 4) return invalid(who, "out_img must be 16-byte aligned, out_depth 4-byte");
     return BG_OK;
 }
 }  // namespace
@@ -1423,11 +1436,7 @@ extern "C" int32_t bg_tsdf_integrate(BgContext *c, void *stream, const BgTsdfGri
     if (!c || !g || !cam || !out_img || !out_depth) return BG_ERR_NULL;
     int32_t r = check_grid(g, "bg_tsdf_integrate");
     if (r != BG_OK) return r;
-    if (w == 0 || h == 0) return invalid("bg_tsdf_integrate", "empty image");
-    if (!(alpha_min > 0.0f && alpha_min <= 1.0f)) return invalid("bg_tsdf_integrate", "alpha_min must be in (0, 1]");
-    if (cam->camera_model > BG_CAMERA_THIN_PRISM_FISHEYE) return invalid("bg_tsdf_integrate", "unknown camera model");
-    if ((uintptr_t)out_img % 16 || (uintptr_t)out_depth % 4)
-        return invalid("bg_tsdf_integrate", "out_img must be 16-byte aligned, out_depth 4-byte");
+    if ((r = check_view(cam, w, h, out_img, out_depth, alpha_min, "bg_tsdf_integrate")) != BG_OK) return r;
     BG_CUDA(cudaSetDevice(c->device));
     BG_CUDA(launch_tsdf_integrate((cudaStream_t)stream, *g, *cam, w, h, out_img, out_depth, alpha_min));
     return BG_OK;
@@ -1478,5 +1487,180 @@ extern "C" int32_t bg_mesh_emit(BgContext *c, void *stream, const BgTsdfGrid *g,
     if (host[0] > max_vertices || host[1] > max_triangles) return capacity("bg_mesh_emit", "the mesh exceeds max_vertices / max_triangles");
     if (host[0] == 0) return BG_OK;   // no vertices, so no triangles
     BG_CUDA(launch_mesh_emit(s, *g, w.voff, w.toff, w.vbase, w.vmask, max_vertices, max_triangles, vertices, colors, faces));
+    return BG_OK;
+}
+
+// ---- Sparse mesh export (mesh_sparse.cu, DESIGN.md section 4.10)
+namespace {
+uint64_t sparse_brick_count(const uint32_t *dims) {
+    return (uint64_t)((dims[0] + 7) / 8) * ((dims[1] + 7) / 8) * ((dims[2] + 7) / 8);
+}
+// w = h = 0: the part kept for the grid's life, without a view's pyramid
+SparseTsdfWs carve_sparse_ws(void *base, const uint32_t *dims, uint32_t w, uint32_t h, uint64_t &bytes) {
+    Carver cv{base};
+    SparseTsdfWs s;
+    const uint64_t nb = sparse_brick_count(dims), nblk = (nb + 1023) / 1024;
+    s.header = cv.take<unsigned long long>(8);
+    s.cand_count = cv.take<uint32_t>(1);
+    s.bitmap = cv.take<uint32_t>((nb + 31) / 32);
+    s.blk_cnt = cv.take<uint32_t>(nblk);
+    s.blk_off = cv.take<uint32_t>(nblk);
+    s.list = cv.take<uint32_t>(nb);
+    s.pyramid = cv.take<float2>(w && h ? sparse_pyramid_cells(w, h) : 0);
+    bytes = cv.off;
+    return s;
+}
+SparseMeshWs carve_sparse_mesh_ws(void *base, uint32_t num_bricks, uint64_t &bytes) {
+    Carver cv{base};
+    SparseMeshWs m;
+    const uint64_t np = (uint64_t)num_bricks * 512;
+    m.header = cv.take<unsigned long long>(8);
+    m.brick_v = cv.take<uint32_t>(num_bricks); m.brick_t = cv.take<uint32_t>(num_bricks);
+    m.voff = cv.take<uint32_t>(num_bricks); m.toff = cv.take<uint32_t>(num_bricks);
+    m.vbase = cv.take<uint32_t>(np);
+    m.vmask = cv.take<uint8_t>(np);
+    bytes = cv.off;
+    return m;
+}
+// The grid and its workspace (sized for a w x h view; 0 x 0 for the calls that take no view).
+int32_t check_sparse_grid(const BgSparseTsdfGrid *g, uint32_t w, uint32_t h, const char *who, SparseTsdfWs &ws) {
+    if (!g->brick_slot) return BG_ERR_NULL;
+    if (!g->dims[0] || !g->dims[1] || !g->dims[2] || g->dims[0] > (1u << 24) || g->dims[1] > (1u << 24) || g->dims[2] > (1u << 24) ||
+        sparse_brick_count(g->dims) >= (1ull << 31))
+        return invalid(who, "grid dims must be in [1, 2^24] with fewer than 2^31 bricks");
+    if ((uintptr_t)g->brick_slot % 4) return invalid(who, "brick_slot must be 4-byte aligned");
+    int32_t r = check_lattice(g->origin, g->h, g->trunc, who);
+    if (r != BG_OK) return r;
+    uint64_t need;
+    ws = carve_sparse_ws(g->workspace, g->dims, w, h, need);
+    return check_workspace(who, "bg_sparse_tsdf_workspace_bytes", g->workspace, g->workspace_bytes, need);
+}
+int32_t check_sparse_pool(const BgSparseTsdfGrid *g, const char *who) {
+    if (g->num_bricks && (!g->tsdf || !g->weight || !g->rgb)) return BG_ERR_NULL;
+    if (((uintptr_t)g->tsdf | (uintptr_t)g->weight | (uintptr_t)g->rgb) % 4) return invalid(who, "pool arrays must be 4-byte aligned");
+    return BG_OK;
+}
+// Reads the grid header back: the allocated brick count, which the pool must hold.
+int32_t sparse_slots(cudaStream_t s, const BgSparseTsdfGrid *g, const SparseTsdfWs &ws, const char *who, uint32_t &slots) {
+    unsigned long long host[8];
+    BG_CUDA(cudaMemcpyAsync(host, ws.header, sizeof(host), cudaMemcpyDeviceToHost, s));
+    BG_CUDA(cudaStreamSynchronize(s));
+    if (!host[SPARSE_H_ALLOCATED]) return invalid(who, "the grid is not allocated (bg_sparse_tsdf_allocate)");
+    if (host[SPARSE_H_DIMS] != g->dims[0] || host[SPARSE_H_DIMS + 1] != g->dims[1] || host[SPARSE_H_DIMS + 2] != g->dims[2])
+        return invalid(who, "the workspace was allocated for a grid with other dims");
+    if (host[SPARSE_H_BRICKS] > g->num_bricks) return capacity(who, "num_bricks is smaller than the allocated brick count");
+    slots = (uint32_t)host[SPARSE_H_BRICKS];
+    return BG_OK;
+}
+}  // namespace
+
+extern "C" uint64_t bg_sparse_tsdf_workspace_bytes(uint32_t dx, uint32_t dy, uint32_t dz, uint32_t max_w, uint32_t max_h) {
+    const uint32_t dims[3] = {std::max(dx, 1u), std::max(dy, 1u), std::max(dz, 1u)};
+    uint64_t bytes;
+    carve_sparse_ws(nullptr, dims, max_w, max_h, bytes);
+    return bytes;
+}
+
+extern "C" int32_t bg_sparse_tsdf_mark(BgContext *c, void *stream, const BgSparseTsdfGrid *g, const BgCamera *cam, uint32_t w,
+                                       uint32_t h, const float *out_img, const float *out_depth, float alpha_min) {
+    if (!c || !g || !cam || !out_img || !out_depth) return BG_ERR_NULL;
+    int32_t r = check_view(cam, w, h, out_img, out_depth, alpha_min, "bg_sparse_tsdf_mark");
+    if (r != BG_OK) return r;
+    SparseTsdfWs ws;
+    if ((r = check_sparse_grid(g, w, h, "bg_sparse_tsdf_mark", ws)) != BG_OK) return r;
+    BG_CUDA(cudaSetDevice(c->device));
+    BG_CUDA(launch_sparse_mark((cudaStream_t)stream, c->sm_count, *g, *cam, w, h, out_img, out_depth, alpha_min, ws));
+    return BG_OK;
+}
+
+extern "C" int32_t bg_sparse_tsdf_allocate(BgContext *c, void *stream, const BgSparseTsdfGrid *g, uint32_t *num_bricks) {
+    if (!c || !g || !num_bricks) return BG_ERR_NULL;
+    *num_bricks = 0;
+    SparseTsdfWs ws;
+    int32_t r = check_sparse_grid(g, 0, 0, "bg_sparse_tsdf_allocate", ws);
+    if (r != BG_OK) return r;
+    cudaStream_t s = (cudaStream_t)stream;
+    BG_CUDA(cudaSetDevice(c->device));
+    BG_CUDA(launch_sparse_allocate(s, *g, ws));
+    unsigned long long host;
+    BG_CUDA(cudaMemcpyAsync(&host, ws.header + SPARSE_H_BRICKS, sizeof(host), cudaMemcpyDeviceToHost, s));
+    BG_CUDA(cudaStreamSynchronize(s));
+    *num_bricks = (uint32_t)host;   // at most the brick count, < 2^31
+    return BG_OK;
+}
+
+extern "C" int32_t bg_sparse_tsdf_integrate(BgContext *c, void *stream, const BgSparseTsdfGrid *g, const BgCamera *cam, uint32_t w,
+                                            uint32_t h, const float *out_img, const float *out_depth, float alpha_min) {
+    if (!c || !g || !cam || !out_img || !out_depth) return BG_ERR_NULL;
+    int32_t r = check_view(cam, w, h, out_img, out_depth, alpha_min, "bg_sparse_tsdf_integrate");
+    if (r != BG_OK) return r;
+    SparseTsdfWs ws;
+    if ((r = check_sparse_grid(g, 0, 0, "bg_sparse_tsdf_integrate", ws)) != BG_OK) return r;
+    if ((r = check_sparse_pool(g, "bg_sparse_tsdf_integrate")) != BG_OK) return r;
+    cudaStream_t s = (cudaStream_t)stream;
+    BG_CUDA(cudaSetDevice(c->device));
+    uint32_t slots;
+    if ((r = sparse_slots(s, g, ws, "bg_sparse_tsdf_integrate", slots)) != BG_OK || slots == 0) return r;
+    BG_CUDA(launch_sparse_integrate(s, *g, slots, *cam, w, h, out_img, out_depth, alpha_min, ws));
+    return BG_OK;
+}
+
+extern "C" uint64_t bg_sparse_mesh_workspace_bytes(uint32_t num_bricks) {
+    uint64_t bytes;
+    carve_sparse_mesh_ws(nullptr, num_bricks, bytes);
+    return bytes;
+}
+
+extern "C" int32_t bg_sparse_mesh_count(BgContext *c, void *stream, const BgSparseTsdfGrid *g, void *mws, uint64_t mws_bytes,
+                                        uint32_t *num_vertices, uint32_t *num_triangles) {
+    if (!c || !g || !num_vertices || !num_triangles) return BG_ERR_NULL;
+    *num_vertices = 0;
+    *num_triangles = 0;
+    SparseTsdfWs ws;
+    int32_t r = check_sparse_grid(g, 0, 0, "bg_sparse_mesh_count", ws);
+    if (r != BG_OK) return r;
+    if ((r = check_sparse_pool(g, "bg_sparse_mesh_count")) != BG_OK) return r;
+    uint64_t need;
+    const SparseMeshWs m = carve_sparse_mesh_ws(mws, g->num_bricks, need);
+    if ((r = check_workspace("bg_sparse_mesh_count", "bg_sparse_mesh_workspace_bytes", mws, mws_bytes, need)) != BG_OK) return r;
+    cudaStream_t s = (cudaStream_t)stream;
+    BG_CUDA(cudaSetDevice(c->device));
+    uint32_t slots;
+    if ((r = sparse_slots(s, g, ws, "bg_sparse_mesh_count", slots)) != BG_OK) return r;
+    BG_CUDA(launch_sparse_mesh_count(s, *g, slots, ws, m));
+    unsigned long long host[2];
+    BG_CUDA(cudaMemcpyAsync(host, m.header, sizeof(host), cudaMemcpyDeviceToHost, s));
+    BG_CUDA(cudaStreamSynchronize(s));
+    if (host[0] > 0xFFFFFFFFull || host[1] > 0xFFFFFFFFull)
+        return capacity("bg_sparse_mesh_count", "more than 2^32 - 1 vertices or triangles");
+    *num_vertices = (uint32_t)host[0];
+    *num_triangles = (uint32_t)host[1];
+    return BG_OK;
+}
+
+extern "C" int32_t bg_sparse_mesh_emit(BgContext *c, void *stream, const BgSparseTsdfGrid *g, void *mws, uint64_t mws_bytes,
+                                       uint32_t max_vertices, uint32_t max_triangles, float *vertices, uint8_t *colors,
+                                       uint32_t *faces) {
+    if (!c || !g) return BG_ERR_NULL;
+    SparseTsdfWs ws;
+    int32_t r = check_sparse_grid(g, 0, 0, "bg_sparse_mesh_emit", ws);
+    if (r != BG_OK) return r;
+    if ((r = check_sparse_pool(g, "bg_sparse_mesh_emit")) != BG_OK) return r;
+    if ((max_vertices && (!vertices || !colors)) || (max_triangles && !faces)) return BG_ERR_NULL;
+    if (((uintptr_t)vertices | (uintptr_t)faces) % 4) return invalid("bg_sparse_mesh_emit", "vertices and faces must be 4-byte aligned");
+    uint64_t need;
+    const SparseMeshWs m = carve_sparse_mesh_ws(mws, g->num_bricks, need);
+    if ((r = check_workspace("bg_sparse_mesh_emit", "bg_sparse_mesh_workspace_bytes", mws, mws_bytes, need)) != BG_OK) return r;
+    cudaStream_t s = (cudaStream_t)stream;
+    BG_CUDA(cudaSetDevice(c->device));
+    unsigned long long host[6];
+    BG_CUDA(cudaMemcpyAsync(host, m.header, sizeof(host), cudaMemcpyDeviceToHost, s));
+    BG_CUDA(cudaStreamSynchronize(s));
+    if (host[3] != g->dims[0] || host[4] != g->dims[1] || host[5] != g->dims[2] || host[2] > g->num_bricks)
+        return invalid("bg_sparse_mesh_emit", "the workspace holds no bg_sparse_mesh_count of a grid with these dims and pool");
+    if (host[0] > max_vertices || host[1] > max_triangles)
+        return capacity("bg_sparse_mesh_emit", "the mesh exceeds max_vertices / max_triangles");
+    if (host[0] == 0) return BG_OK;   // no vertices, so no triangles
+    BG_CUDA(launch_sparse_mesh_emit(s, *g, (uint32_t)host[2], ws, m, max_vertices, max_triangles, vertices, colors, faces));
     return BG_OK;
 }

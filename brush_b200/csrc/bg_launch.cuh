@@ -183,6 +183,38 @@ cudaError_t launch_mesh_emit(cudaStream_t s, const BgTsdfGrid &g, const uint32_t
                              uint8_t *vmask, uint32_t max_vertices, uint32_t max_triangles, float *verts, uint8_t *colors,
                              uint32_t *faces);
 
+// ---- mesh_sparse.cu
+// The grid workspace (bg_sparse_tsdf_workspace_bytes): header [8] u64 (allocated bricks, -, allocated flag, dims),
+// the candidate count, the mark bitmap [ceil(bricks / 32)], per-1024-brick counts and offsets, `list` [bricks] (the
+// candidates of the view being marked, then the brick of every slot) and the view's expected-depth pyramid.
+constexpr uint32_t SPARSE_H_BRICKS = 0, SPARSE_H_ALLOCATED = 2, SPARSE_H_DIMS = 3;
+struct SparseTsdfWs {
+    unsigned long long *header;
+    uint32_t *cand_count, *bitmap, *blk_cnt, *blk_off, *list;
+    float2 *pyramid;
+};
+// The extraction workspace (bg_sparse_mesh_workspace_bytes): header [8] u64 (vertex total, triangle total, slots counted,
+// dims), per-slot counts and offsets, and each pool point's vertex base and edge mask.
+struct SparseMeshWs {
+    unsigned long long *header;
+    uint32_t *brick_v, *brick_t, *voff, *toff, *vbase;
+    uint8_t *vmask;
+};
+uint64_t sparse_pyramid_cells(uint32_t w, uint32_t h);
+// img: float4 [h,w], depth [h,w]: ORs the bricks holding a point that this view updates with f < 0 into the bitmap
+cudaError_t launch_sparse_mark(cudaStream_t s, int sm_count, const BgSparseTsdfGrid &g, const BgCamera &cam, uint32_t w, uint32_t h,
+                               const float *img, const float *depth, float alpha_min, const SparseTsdfWs &ws);
+// Dilates the bitmap by one brick, writes g.brick_slot and the brick of every slot, header[SPARSE_H_BRICKS] = the count
+cudaError_t launch_sparse_allocate(cudaStream_t s, const BgSparseTsdfGrid &g, const SparseTsdfWs &ws);
+// slots: the allocated count (<= g.num_bricks)
+cudaError_t launch_sparse_integrate(cudaStream_t s, const BgSparseTsdfGrid &g, uint32_t slots, const BgCamera &cam, uint32_t w,
+                                    uint32_t h, const float *img, const float *depth, float alpha_min, const SparseTsdfWs &ws);
+cudaError_t launch_sparse_mesh_count(cudaStream_t s, const BgSparseTsdfGrid &g, uint32_t slots, const SparseTsdfWs &ws,
+                                     const SparseMeshWs &m);
+cudaError_t launch_sparse_mesh_emit(cudaStream_t s, const BgSparseTsdfGrid &g, uint32_t slots, const SparseTsdfWs &ws,
+                                    const SparseMeshWs &m, uint32_t max_vertices, uint32_t max_triangles, float *verts,
+                                    uint8_t *colors, uint32_t *faces);
+
 // ---- depth_loss.cu
 uint32_t depth_loss_num_partials(uint32_t h, uint32_t w);
 // out_img / v_output: float4 [h,w]; adds the depth term's gradient to v_output[..., 3], writes v_depth [h,w] and

@@ -439,6 +439,50 @@ int32_t bg_mesh_count(BgContext *ctx, void *stream, const BgTsdfGrid *grid, void
 int32_t bg_mesh_emit(BgContext *ctx, void *stream, const BgTsdfGrid *grid, void *workspace, uint64_t workspace_bytes,
                      uint32_t max_vertices, uint32_t max_triangles, float *vertices, uint8_t *colors, uint32_t *faces);
 
+/* ---- Sparse mesh export (DESIGN.md section 4.10): the same lattice and arithmetic as BgTsdfGrid, stored only in the
+ * 8^3-point bricks within one brick of a point that some view updates with f < 0.  Its mesh equals the dense grid's over
+ * the same lattice bit for bit and in the same order; memory follows the surface, so lattices far past 2^31 points fit.
+ * Bricks (bx, by, bz) = (i/8, j/8, k/8), linear index (bz * nby + by) * nbx + bx with nb* = ceil(dims / 8); at most
+ * 2^31 - 1 bricks and at most 2^24 points per axis.  Phases, in this order:
+ * bg_sparse_tsdf_mark, once per view before any integration, with the render bg_tsdf_integrate would take (black
+ *     background; any camera model).  Marks every brick holding a point that the view updates with f < 0.  After
+ *     bg_sparse_tsdf_allocate it changes nothing.
+ * bg_sparse_tsdf_allocate (blocking: one readback) grows the marked set by one brick in every direction, writes
+ *     brick_slot [nb] (u32: slot, 0xFFFFFFFF = unallocated; slots in linear brick order) and returns the count in
+ *     *num_bricks.  The caller then allocates and zeroes the pool: tsdf, weight [count, 512] and rgb [count, 512, 3],
+ *     point (x, y, z) of a brick at x + 8 y + 64 z.
+ * bg_sparse_tsdf_integrate fuses one view into every allocated point exactly as bg_tsdf_integrate would (blocking:
+ *     it reads the allocated count back); BG_ERR_INVALID before the allocation, BG_ERR_CAPACITY when num_bricks is
+ *     smaller than the count.
+ * bg_sparse_mesh_count / bg_sparse_mesh_emit: bg_mesh_count / bg_mesh_emit over the allocated bricks, with a workspace of
+ *     bg_sparse_mesh_workspace_bytes(num_bricks); unallocated points read as unobserved.
+ * workspace: bg_sparse_tsdf_workspace_bytes(dims, max_w, max_h) for views up to max_w x max_h, 256-byte aligned, zeroed
+ *     at creation and kept for the grid's life. */
+typedef struct {
+    float origin[3];
+    float h;                    /* lattice spacing */
+    uint32_t dims[3];           /* dx, dy, dz (points) */
+    float trunc;                /* truncation distance, scene units */
+    uint32_t *brick_slot;       /* [nbz, nby, nbx], written by bg_sparse_tsdf_allocate */
+    void *workspace;
+    uint64_t workspace_bytes;
+    uint32_t num_bricks;        /* pool capacity in bricks */
+    float *tsdf;                /* [num_bricks, 512] */
+    float *weight;              /* [num_bricks, 512] */
+    float *rgb;                 /* [num_bricks, 512, 3] */
+} BgSparseTsdfGrid;
+uint64_t bg_sparse_tsdf_workspace_bytes(uint32_t dx, uint32_t dy, uint32_t dz, uint32_t max_w, uint32_t max_h);
+int32_t bg_sparse_tsdf_mark(BgContext *ctx, void *stream, const BgSparseTsdfGrid *grid, const BgCamera *cam, uint32_t w,
+                            uint32_t h, const float *out_img, const float *out_depth, float alpha_min);
+int32_t bg_sparse_tsdf_allocate(BgContext *ctx, void *stream, const BgSparseTsdfGrid *grid, uint32_t *num_bricks /* host */);
+int32_t bg_sparse_tsdf_integrate(BgContext *ctx, void *stream, const BgSparseTsdfGrid *grid, const BgCamera *cam, uint32_t w,
+                                 uint32_t h, const float *out_img, const float *out_depth, float alpha_min);
+uint64_t bg_sparse_mesh_workspace_bytes(uint32_t num_bricks);
+int32_t bg_sparse_mesh_count(BgContext *ctx, void *stream, const BgSparseTsdfGrid *grid, void *workspace,
+                             uint64_t workspace_bytes, uint32_t *num_vertices /* host */, uint32_t *num_triangles /* host */);
+int32_t bg_sparse_mesh_emit(BgContext *ctx, void *stream, const BgSparseTsdfGrid *grid, void *workspace, uint64_t workspace_bytes,
+                            uint32_t max_vertices, uint32_t max_triangles, float *vertices, uint8_t *colors, uint32_t *faces);
+
 /* ---- View-sharded data parallelism behind the boundary (SURVEY.md section 8e; the reference is single-device).
  * A communicator is one NCCL rank bound to the context's device.  Rank 0 calls bg_dp_unique_id and ships the 128 bytes
  * to the other ranks by any side channel (the Python mirror uses torch.distributed's store; a Rust host would use

@@ -20,6 +20,7 @@
 //   pup_scores, decimate_to_count <- LOD baking, brush-train/src/lod.rs:13-142 (bg_pup_*, bg_decimate_to_count)
 //   compress_splats, compressed_ply_bytes <- SuperSplat compressed PLY export (bg_compress_splats; the reference only reads
 //                                  the layout, brush-serde/src/import.rs:408-600)
+//   SparseTsdfGrid, sparse_tsdf_mark / _allocate / _integrate, extract_mesh <- the sparse brick grid (bg_sparse_*; 4.10)
 //   TsdfGrid, tsdf_integrate, extract_mesh, mesh_ply_bytes <- mesh export (bg_tsdf_integrate, bg_mesh_count, bg_mesh_emit;
 //                                  no reference counterpart, DESIGN.md section 4.9)
 //
@@ -971,6 +972,74 @@ inline TriangleMesh extract_mesh(Context &ctx, cudaStream_t stream, const TsdfGr
     DeviceBuffer<uint8_t> c((size_t)nv * 3);
     DeviceBuffer<uint32_t> f((size_t)nt * 3);
     check(bg_mesh_emit(ctx.handle(), stream, &g.grid, ws.data(), need, nv, nt, v.data(), c.data(), f.data()), "extract_mesh: emit");
+    TriangleMesh m;
+    m.vertices.resize((size_t)nv * 3); m.colors.resize((size_t)nv * 3); m.faces.resize((size_t)nt * 3);
+    if (nv) { v.download(m.vertices.data(), m.vertices.size(), stream); c.download(m.colors.data(), m.colors.size(), stream); }
+    if (nt) f.download(m.faces.data(), m.faces.size(), stream);
+    return m;
+}
+
+// The sparse brick grid over the same lattice (DESIGN.md section 4.10): mark every view, allocate once, integrate every
+// view, extract; the mesh equals the dense grid's bit for bit.  Views up to max_w x max_h.
+struct SparseTsdfGrid {
+    BgSparseTsdfGrid grid;
+    DeviceBuffer<uint32_t> brick_slot;
+    DeviceBuffer<unsigned char> workspace;
+    DeviceBuffer<float> tsdf, weight, rgb;
+    bool allocated = false;
+    SparseTsdfGrid(const float origin[3], float h, const uint32_t dims[3], float trunc, uint32_t max_w, uint32_t max_h) {
+        const uint64_t nb = (uint64_t)((dims[0] + 7) / 8) * ((dims[1] + 7) / 8) * ((dims[2] + 7) / 8);
+        if (nb == 0 || nb >= (1ull << 31)) throw Error(BG_ERR_INVALID, "SparseTsdfGrid: dims must be non-zero with fewer than 2^31 bricks");
+        const uint64_t ws = bg_sparse_tsdf_workspace_bytes(dims[0], dims[1], dims[2], max_w, max_h);
+        brick_slot = DeviceBuffer<uint32_t>(nb);
+        workspace = DeviceBuffer<unsigned char>(ws, true);
+        std::memset(&grid, 0, sizeof(grid));
+        for (int a = 0; a < 3; a++) { grid.origin[a] = origin[a]; grid.dims[a] = dims[a]; }
+        grid.h = h;
+        grid.trunc = trunc;
+        grid.brick_slot = brick_slot.data();
+        grid.workspace = workspace.data();
+        grid.workspace_bytes = ws;
+    }
+};
+
+// Marks the bricks one view (a render_splats_depth output on a black background) updates with f < 0.  Before allocation.
+inline void sparse_tsdf_mark(Context &ctx, cudaStream_t stream, SparseTsdfGrid &g, const BgCamera &cam, uint32_t w, uint32_t h,
+                             const float *out_img, const float *out_depth, float alpha_min = 0.5f) {
+    if (g.allocated) throw Error(BG_ERR_INVALID, "sparse_tsdf_mark: the grid is already allocated");
+    check(bg_sparse_tsdf_mark(ctx.handle(), stream, &g.grid, &cam, w, h, out_img, out_depth, alpha_min), "sparse_tsdf_mark");
+}
+
+// Allocates the marked bricks and their neighbours and a zeroed pool for them; returns the brick count.
+inline uint32_t sparse_tsdf_allocate(Context &ctx, cudaStream_t stream, SparseTsdfGrid &g) {
+    if (g.allocated) throw Error(BG_ERR_INVALID, "sparse_tsdf_allocate: the grid is already allocated");
+    uint32_t n = 0;
+    check(bg_sparse_tsdf_allocate(ctx.handle(), stream, &g.grid, &n), "sparse_tsdf_allocate");
+    g.tsdf = DeviceBuffer<float>((size_t)n * 512, true);
+    g.weight = DeviceBuffer<float>((size_t)n * 512, true);
+    g.rgb = DeviceBuffer<float>((size_t)n * 512 * 3, true);
+    g.grid.num_bricks = n;
+    g.grid.tsdf = g.tsdf.data(); g.grid.weight = g.weight.data(); g.grid.rgb = g.rgb.data();
+    g.allocated = true;
+    return n;
+}
+
+inline void sparse_tsdf_integrate(Context &ctx, cudaStream_t stream, SparseTsdfGrid &g, const BgCamera &cam, uint32_t w,
+                                  uint32_t h, const float *out_img, const float *out_depth, float alpha_min = 0.5f) {
+    check(bg_sparse_tsdf_integrate(ctx.handle(), stream, &g.grid, &cam, w, h, out_img, out_depth, alpha_min),
+          "sparse_tsdf_integrate");
+}
+
+inline TriangleMesh extract_mesh(Context &ctx, cudaStream_t stream, const SparseTsdfGrid &g) {
+    const uint64_t need = bg_sparse_mesh_workspace_bytes(g.grid.num_bricks);
+    DeviceBuffer<unsigned char> ws(need);
+    uint32_t nv = 0, nt = 0;
+    check(bg_sparse_mesh_count(ctx.handle(), stream, &g.grid, ws.data(), need, &nv, &nt), "extract_mesh: sparse count");
+    DeviceBuffer<float> v((size_t)nv * 3);
+    DeviceBuffer<uint8_t> c((size_t)nv * 3);
+    DeviceBuffer<uint32_t> f((size_t)nt * 3);
+    check(bg_sparse_mesh_emit(ctx.handle(), stream, &g.grid, ws.data(), need, nv, nt, v.data(), c.data(), f.data()),
+          "extract_mesh: sparse emit");
     TriangleMesh m;
     m.vertices.resize((size_t)nv * 3); m.colors.resize((size_t)nv * 3); m.faces.resize((size_t)nt * 3);
     if (nv) { v.download(m.vertices.data(), m.vertices.size(), stream); c.download(m.colors.data(), m.colors.size(), stream); }
