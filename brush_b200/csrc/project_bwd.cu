@@ -136,6 +136,13 @@ __device__ __forceinline__ V3 sh_viewdir_vjp(const float *S, V3 v) {
 }
 
 constexpr int PB_THREADS = 128;
+constexpr int PB_WARPS = PB_THREADS / 32;
+
+// Row stride, in floats, of the per-warp SH slices in shared memory.  Rows that are a multiple of 16 bytes are
+// accessed with 128-bit shared loads and stores, which run in phases of 8 lanes: an odd number of float4s per row puts
+// those 8 lanes on 8 distinct 4-bank groups, so KF = 12 stays as it is and KF = 48 is padded to 52.  Odd rows
+// (KF = 3, 27, 75) are accessed one float at a time, which an odd stride keeps conflict-free.
+__host__ __device__ constexpr int pb_slice_stride(int kf) { return (kf % 4 != 0 || (kf / 4) % 2 == 1) ? kf : kf + 4; }
 
 template <bool MIP, int DEG, bool DIST>
 __global__ void __launch_bounds__(PB_THREADS)
@@ -146,15 +153,34 @@ project_bwd_kernel(const float *__restrict__ transforms, const float *__restrict
                    float *__restrict__ v_color_out /* nullable: factored mode, see sh_grad_from_views_kernel */) {
     constexpr int K = (DEG + 1) * (DEG + 1);
     constexpr int KF = K * 3;
-    // SH rows in and SH gradient rows out go straight between registers and global memory, one row per thread
-    // (128-bit accesses when the row is a multiple of 16 bytes): consecutive threads own consecutive rows, so a
-    // warp's 12 accesses cover one contiguous 6 KB span and every fetched sector is used out of L1.
+    // The SH rows move through a shared-memory slice of 32 rows per warp, so that neither direction makes a warp
+    // touch 32 different 128-byte lines per instruction, as one row per thread straight from global memory would.
+    //   in:  a row that is a multiple of 16 bytes (K = 4, 16) comes in by its own TMA bulk copy (cp.async.bulk, SASS
+    //        UBLKCP), issued by one lane per warp as soon as the v_combined gather says the row is read at all, and
+    //        lands while the transform row and the projection chain are worked through.  Culled and zero-gradient
+    //        rows are never fetched.  Odd rows (K = 9, 25) keep the per-thread load.
+    //   out: each lane leaves its SH-gradient row (zeros included) in its slot, then the warp writes its contiguous
+    //        32-row span with whole-line stores (degree >= 1; a degree-0 row goes straight out).
     constexpr bool VEC4 = (KF % 4) == 0;
+    constexpr bool BULK_IN = VEC4 && DEG > 0;   // degree 0 has no view-direction dependence: its row is never read
+    // degree 0 rows are 12 bytes: a warp's direct stores of them already cover one contiguous 384-byte span
+    constexpr bool STAGE_OUT = DEG > 0;
+    constexpr int ST = pb_slice_stride(KF);
     __shared__ __align__(16) float s_vt[PB_THREADS * 10];
+    __shared__ __align__(16) float s_sh[PB_THREADS * ST];
+    __shared__ unsigned long long s_bar[PB_WARPS];
     const uint32_t base = blockIdx.x * PB_THREADS;
     const uint32_t rows = min((uint32_t)PB_THREADS, n - base);
     const uint32_t gid = base + threadIdx.x;
     const bool in_range = threadIdx.x < rows;
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    const uint32_t wbase = base + warp * 32u;   // first Gaussian of this warp's slice
+    float *slice = s_sh + warp * 32u * ST;
+    float *my_row = slice + lane * ST;
+    if (BULK_IN) {
+        if (lane == 0) mbar_init(&s_bar[warp], 1);
+        __syncwarp();
+    }
 
     uint32_t cg = 0xFFFFFFFFu;
     float rg[10];
@@ -171,6 +197,17 @@ project_bwd_kernel(const float *__restrict__ transforms, const float *__restrict
     bool any = false;
 #pragma unroll
     for (int i = 0; i < 10; i++) any = any || (rg[i] != 0.0f);
+    if (BULK_IN) {
+        const uint32_t mask = __ballot_sync(0xffffffffu, any);
+        if (lane == 0 && mask != 0u) {
+            const float *src = sh + (size_t)wbase * KF;
+            mbar_expect_tx(&s_bar[warp], (uint32_t)__popc(mask) * (KF * 4u));
+            for (uint32_t m = mask; m != 0u; m &= m - 1u) {
+                const uint32_t r = (uint32_t)__ffs(m) - 1u;
+                tma_bulk_g2s(slice + r * ST, src + (size_t)r * KF, KF * 4u, &s_bar[warp]);
+            }
+        }
+    }
 
     float vt[10];
 #pragma unroll
@@ -193,28 +230,6 @@ project_bwd_kernel(const float *__restrict__ transforms, const float *__restrict
         float u_len = length(u_world);
         V3 vdir = scale(u_world, 1.0f / u_len);
         sh_basis<DEG>(vdir, Y);
-        float S[K];
-        if (DEG > 0) {   // S_k = coeff_k . v_color; degree 0 has no view-direction dependence: its row is never read
-            float row[KF];
-            const float *src = sh + (size_t)gid * KF;
-            if (VEC4) {
-#pragma unroll
-                for (int q = 0; q < KF / 4; q++) {
-                    float4 t = __ldg(reinterpret_cast<const float4 *>(src) + q);
-                    row[4 * q] = t.x; row[4 * q + 1] = t.y; row[4 * q + 2] = t.z; row[4 * q + 3] = t.w;
-                }
-            } else {
-#pragma unroll
-                for (int q = 0; q < KF; q++) row[q] = __ldg(src + q);
-            }
-#pragma unroll
-            for (int k = 0; k < K; k++) S[k] = dot(mk3(row[3 * k], row[3 * k + 1], row[3 * k + 2]), v_color);
-        } else {
-            S[0] = 0.0f;
-        }
-        V3 v_v_sh = sh_viewdir_vjp<DEG>(S, vdir);
-        float vdv = dot(vdir, v_v_sh);
-        V3 v_mean_sh = scale(sub(v_v_sh, scale(vdir, vdv)), 1.0f / u_len);
 
         V3 mean_c = world_to_cam(mean, u);
         M3 rm = quat_to_mat3(quat);
@@ -237,6 +252,32 @@ project_bwd_kernel(const float *__restrict__ transforms, const float *__restrict
         V3 v_mean_c = DIST ? projection_vjp_distorted(jac, mean_c, cov_c, u, v_cov2d, mk2(rg[0], rg[1]))
                            : projection_vjp_pinhole(jac, mean_c, cov_c, u, v_cov2d, mk2(rg[0], rg[1]));
         S3 vcc = tcongruence(jac, v_cov2d);
+
+        // the SH row is needed only from here on, which gives its bulk copy the whole chain above to land
+        float S[K];
+        if (DEG > 0) {   // S_k = coeff_k . v_color
+            float row[KF];
+            if (BULK_IN) {
+                mbar_wait(&s_bar[warp], 0);
+#pragma unroll
+                for (int q = 0; q < KF / 4; q++) {
+                    float4 t = reinterpret_cast<const float4 *>(my_row)[q];
+                    row[4 * q] = t.x; row[4 * q + 1] = t.y; row[4 * q + 2] = t.z; row[4 * q + 3] = t.w;
+                }
+            } else {
+                const float *src = sh + (size_t)gid * KF;
+#pragma unroll
+                for (int q = 0; q < KF; q++) row[q] = __ldg(src + q);
+            }
+#pragma unroll
+            for (int k = 0; k < K; k++) S[k] = dot(mk3(row[3 * k], row[3 * k + 1], row[3 * k + 2]), v_color);
+        } else {
+            S[0] = 0.0f;
+        }
+        V3 v_v_sh = sh_viewdir_vjp<DEG>(S, vdir);
+        float vdv = dot(vdir, v_v_sh);
+        V3 v_mean_sh = scale(sub(v_v_sh, scale(vdir, vdv)), 1.0f / u_len);
+
         V3 v_mean = add(tmul(view_rot, v_mean_c), v_mean_sh);
         M3 v_m = mul(scale(tcongruence(vcc, view_rot), 2.0f), m);
         V3 v_scale = mk3(dot(rm.c0, v_m.c0) * scl.x, dot(rm.c1, v_m.c1) * scl.y, dot(rm.c2, v_m.c2) * scl.z);
@@ -247,8 +288,16 @@ project_bwd_kernel(const float *__restrict__ transforms, const float *__restrict
         vt[7] = v_scale.x; vt[8] = v_scale.y; vt[9] = v_scale.z;
     }
     const bool factored = v_color_out != nullptr;
-    if (in_range) {
-        if (!factored) {
+    if (!factored && !STAGE_OUT) {
+        if (in_range) {
+            float *dst = v_sh + (size_t)gid * KF;
+            const float yk = any ? Y[0] : 0.0f;
+            dst[0] = v_color.x * yk; dst[1] = v_color.y * yk; dst[2] = v_color.z * yk;
+        }
+    } else if (!factored) {
+        // this lane's row of the dense gradient into its slot (a row it read above has been consumed by then), then
+        // the warp's rows out as one contiguous span
+        if (in_range) {
             float row[KF];
 #pragma unroll
             for (int k = 0; k < K; k++) {
@@ -257,19 +306,36 @@ project_bwd_kernel(const float *__restrict__ transforms, const float *__restrict
                 row[3 * k + 1] = v_color.y * yk;
                 row[3 * k + 2] = v_color.z * yk;
             }
-            float *dst = v_sh + (size_t)gid * KF;
             if (VEC4) {
 #pragma unroll
                 for (int q = 0; q < KF / 4; q++)
-                    reinterpret_cast<float4 *>(dst)[q] = make_float4(row[4 * q], row[4 * q + 1], row[4 * q + 2], row[4 * q + 3]);
+                    reinterpret_cast<float4 *>(my_row)[q] = make_float4(row[4 * q], row[4 * q + 1], row[4 * q + 2], row[4 * q + 3]);
             } else {
 #pragma unroll
-                for (int q = 0; q < KF; q++) dst[q] = row[q];
+                for (int q = 0; q < KF; q++) my_row[q] = row[q];
             }
-        } else {  // the SH gradient of one view is the outer product Y(dir) x v_color: ship only v_color
-            float *dst = v_color_out + (size_t)gid * 3;
-            dst[0] = any ? v_color.x : 0.0f; dst[1] = any ? v_color.y : 0.0f; dst[2] = any ? v_color.z : 0.0f;
         }
+        __syncwarp();
+        if (wbase < n) {
+            const uint32_t wrows = min(32u, n - wbase);
+            float *dst = v_sh + (size_t)wbase * KF;
+            if (VEC4) {   // 16-byte aligned: v_sh is, and the span starts 32 * KF floats into it
+                constexpr uint32_t Q = KF / 4;
+#pragma unroll 4
+                for (uint32_t f = lane; f < wrows * Q; f += 32u) {
+                    const uint32_t r = f / Q, c = f - r * Q;
+                    reinterpret_cast<float4 *>(dst)[f] = *reinterpret_cast<const float4 *>(slice + r * ST + 4u * c);
+                }
+            } else {      // odd rows are stored unpadded: the slot layout is the span's
+#pragma unroll 4
+                for (uint32_t j = lane; j < wrows * KF; j += 32u) dst[j] = slice[j];
+            }
+        }
+    } else if (in_range) {  // the SH gradient of one view is the outer product Y(dir) x v_color: ship only v_color
+        float *dst = v_color_out + (size_t)gid * 3;
+        dst[0] = any ? v_color.x : 0.0f; dst[1] = any ? v_color.y : 0.0f; dst[2] = any ? v_color.z : 0.0f;
+    }
+    if (in_range) {
 #pragma unroll
         for (int i = 0; i < 10; i++) s_vt[threadIdx.x * 10 + i] = vt[i];
         v_raw_opac[gid] = v_opac_out;
