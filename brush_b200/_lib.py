@@ -16,7 +16,9 @@ BG_OK, BG_ERR_NULL, BG_ERR_INVALID, BG_ERR_CUDA, BG_ERR_CAPACITY, BG_ERR_UNSUPPO
 PASS_FORWARD, PASS_BACKWARD, PASS_BACKWARD_SMOOTH = 0, 1, 2
 PROJECTED_STRIDE = 16
 VCOMBINED_STRIDE = 10
-ABI_VERSION = 11
+ABI_VERSION = 12
+BILAGRID_L, BILAGRID_H, BILAGRID_W = 8, 16, 16
+BILAGRID_FLOATS = BILAGRID_L * BILAGRID_H * BILAGRID_W * 12
 
 _STATUS_NAMES = {1: "BG_ERR_NULL", 2: "BG_ERR_INVALID", 3: "BG_ERR_CUDA", 4: "BG_ERR_CAPACITY", 5: "BG_ERR_UNSUPPORTED"}
 
@@ -213,6 +215,15 @@ class BgTrainViewsArgs(C.Structure):
     ]
 
 
+class BgBilagridStep(C.Structure):
+    _fields_ = [
+        ("grid", C.c_void_p), ("m", C.c_void_p), ("v", C.c_void_p),
+        ("step", C.c_int32),
+        ("lr", C.c_float), ("tv_weight", C.c_float),
+        ("tv_loss_out", C.c_void_p),
+    ]
+
+
 # name -> (restype, argtypes); one entry per function declared in include/brush_b200.h
 _P, _U32, _U64, _I32, _I64, _F = C.c_void_p, C.c_uint32, C.c_uint64, C.c_int32, C.c_int64, C.c_float
 SIGNATURES = {
@@ -285,6 +296,11 @@ SIGNATURES = {
     "bg_sparse_mesh_workspace_bytes": (_U64, [_U32]),
     "bg_sparse_mesh_count": (_I32, [_P, _P, C.POINTER(BgSparseTsdfGrid), _P, _U64, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
     "bg_sparse_mesh_emit": (_I32, [_P, _P, C.POINTER(BgSparseTsdfGrid), _P, _U64, _U32, _U32, _P, _P, _P]),
+    "bg_bilagrid_slice": (_I32, [_P, _P, _P, _P, _U32, _U32, _P]),
+    "bg_bilagrid_slice_backward": (_I32, [_P, _P, _P, _P, _P, _U32, _U32, _P, _P]),
+    "bg_bilagrid_update": (_I32, [_P, _P, C.POINTER(BgBilagridStep), _P]),
+    "bg_train_step_bilagrid_workspace_bytes": (_U64, [_U32, _U32, _U32, _U32]),
+    "bg_train_step_bilagrid": (_I32, [_P, _P, C.POINTER(BgTrainStepArgs), C.POINTER(BgDepthSupervision), C.POINTER(BgBilagridStep)]),
 }
 
 _lib = None

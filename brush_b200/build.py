@@ -38,6 +38,7 @@ SOURCES = {
     "compress.cu": ["-fmad=false"],
     "mesh.cu": ["-fmad=false"],
     "mesh_sparse.cu": ["-fmad=false"],
+    "bilagrid.cu": [],
 }
 
 

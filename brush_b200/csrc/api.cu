@@ -785,17 +785,17 @@ int32_t check_depth(const BgDepthSupervision &d, const char *who) {
     return BG_OK;
 }
 
-// The loss of one rendered view into *loss (train.rs:220-260): the mean over [h,w,3] (+ alpha mean * weight), value and
-// gradient (into ws.v_output) from the fused kernel.  With d, also the depth term: v_depth, v_output[...,3] += dL/da,
-// L_d -> d->depth_loss_out and added to *loss.
+// The loss of one rendered view into *loss (train.rs:220-260): the mean over [h,w,3] (+ alpha mean * weight) of `img`
+// (ws.out_img, or its bilateral-grid slice), value and gradient (into ws.v_output) from the fused kernel.  With d, also
+// the depth term on the raw render: v_depth, v_output[...,3] += dL/da, L_d -> d->depth_loss_out and added to *loss.
 template <class A, class W>
-int32_t view_loss(BgContext *c, void *stream, const A *a, const uint32_t *gt, const W &ws, float *loss,
+int32_t view_loss(BgContext *c, void *stream, const A *a, const uint32_t *gt, const W &ws, const float *img, float *loss,
                   const BgDepthSupervision *d, const DepthWs &dws) {
     cudaStream_t s = (cudaStream_t)stream;
     const uint32_t w = a->w, h = a->h;
     const float npx = (float)w * (float)h;
     float chain[4] = {1.0f / (3.0f * npx), 1.0f / (3.0f * npx), 1.0f / (3.0f * npx), a->channels == 4 ? a->alpha_weight / npx : 0.0f};
-    int32_t r = bg_image_loss_fused(c, stream, ws.out_img, gt, a->channels, h, w, 1, (int64_t)w * 4, 4, a->l1_weight, a->ssim_weight,
+    int32_t r = bg_image_loss_fused(c, stream, img, gt, a->channels, h, w, 1, (int64_t)w * 4, 4, a->l1_weight, a->ssim_weight,
                                     a->has_composite_bg ? a->composite_bg : nullptr, a->mask, chain, ws.v_output, ws.partials);
     if (r != BG_OK) return r;
     BG_CUDA(launch_loss_reduce(s, ws.partials, a->channels, bg_image_loss_num_partials(a->channels, h, w) / a->channels, chain, loss));
@@ -805,6 +805,45 @@ int32_t view_loss(BgContext *c, void *stream, const A *a, const uint32_t *gt, co
     if (r != BG_OK) return r;
     BG_CUDA(launch_depth_loss_reduce(s, dws.partials, depth_loss_num_partials(h, w), dchain, d->depth_loss_out, loss));
     return BG_OK;
+}
+
+bool aligned16(const void *p) { return (uintptr_t)p % 16 == 0; }
+// whether two [h,w,4] f32 images share any byte
+bool overlap(const float *a, const float *b, uint32_t h, uint32_t w) {
+    const uintptr_t n = (uintptr_t)h * w * 4 * sizeof(float), pa = (uintptr_t)a, pb = (uintptr_t)b;
+    return pa < pb + n && pb < pa + n;
+}
+
+int32_t check_bilagrid_step(const BgBilagridStep *b, const char *who) {
+    if (!b || !b->grid || !b->m || !b->v || !b->tv_loss_out) return BG_ERR_NULL;
+    if (b->step < 1) return invalid(who, "bilateral grid step is 1-based");
+    if (!(b->lr >= 0.0f) || !std::isfinite(b->lr) || !(b->tv_weight >= 0.0f) || !std::isfinite(b->tv_weight))
+        return invalid(who, "bilateral grid lr and tv_weight must be finite and >= 0");
+    if (!aligned16(b->grid) || !aligned16(b->m) || !aligned16(b->v)) return invalid(who, "grid, m and v must be 16-byte aligned");
+    return BG_OK;
+}
+
+// TV into v_grid and *tv_loss_out (and *loss_out when not null), then Adam on the grid (DESIGN.md section 4.11)
+cudaError_t bilagrid_update(cudaStream_t s, const BgBilagridStep *b, float *v_grid, float *loss_out) {
+    cudaError_t e = launch_bilagrid_tv(s, b->grid, v_grid, b->tv_weight, b->tv_loss_out, loss_out);
+    if (e != cudaSuccess) return e;
+    const float beta1 = 0.9f, beta2 = 0.999f;
+    return launch_adam(s, b->grid, v_grid, b->m, b->v, BG_BILAGRID_FLOATS / 4, 4, nullptr, b->lr, beta1, beta2, 1e-15f,
+                       1.0f - powi_f32(beta1, b->step), 1.0f - powi_f32(beta2, b->step), b->step == 1, false);
+}
+
+// the bilateral grid's scratch of bg_train_step_bilagrid, behind the depth step's workspace
+struct BilagridWs {
+    float *sliced, *v_grid;
+    uint64_t bytes;
+};
+BilagridWs carve_bilagrid_ws(void *base, uint64_t off, uint32_t w, uint32_t h) {
+    Carver cv{base, off};
+    BilagridWs ws;
+    ws.sliced = cv.take((uint64_t)w * h * 4);
+    ws.v_grid = cv.take(BG_BILAGRID_FLOATS);
+    ws.bytes = cv.off;
+    return ws;
 }
 }  // namespace
 
@@ -816,17 +855,24 @@ extern "C" uint64_t bg_train_step_depth_workspace_bytes(uint32_t n, uint32_t k, 
     return carve_depth_ws(nullptr, bg_train_step_workspace_bytes(n, k, w, h), n, w, h).bytes;
 }
 
+extern "C" uint64_t bg_train_step_bilagrid_workspace_bytes(uint32_t n, uint32_t k, uint32_t w, uint32_t h) {
+    return carve_bilagrid_ws(nullptr, bg_train_step_depth_workspace_bytes(n, k, w, h), w, h).bytes;
+}
+
 // The single-view step.  d == nullptr: bg_train_step.  Otherwise the step with the depth term of DESIGN.md section 4.7
-// (d validated, its term on, by bg_train_step_depth).
-static int32_t train_step(BgContext *c, void *stream, BgTrainStepArgs *a, const BgDepthSupervision *d) {
-    const char *who = d ? "bg_train_step_depth" : "bg_train_step";
+// (d validated, its term on, by bg_train_step_depth).  bl: the view's bilateral grid (DESIGN.md section 4.11, validated
+// by bg_train_step_bilagrid) or null.
+static int32_t train_step(BgContext *c, void *stream, BgTrainStepArgs *a, const BgDepthSupervision *d, const BgBilagridStep *bl) {
+    const char *who = bl ? "bg_train_step_bilagrid" : d ? "bg_train_step_depth" : "bg_train_step";
     if (int32_t r = check_train_args(a, who); r != BG_OK) return r;
     const uint32_t n = a->n, k = a->k, w = a->w, h = a->h;
     const TrainWs ws = carve_train_ws(a->workspace, n, k, w, h, a->channels);
     // the depth term's buffers; all null without the term, which selects the plain render and blend backward
     const DepthWs dws = carve_depth_ws(d ? a->workspace : nullptr, bg_train_step_workspace_bytes(n, k, w, h), n, w, h);
-    if (int32_t r = check_workspace_bytes(who, d ? "bg_train_step_depth_workspace_bytes" : "bg_train_step_workspace_bytes",
-                                          a->workspace_bytes, d ? dws.bytes : ws.bytes); r != BG_OK) return r;
+    const BilagridWs bws = carve_bilagrid_ws(bl ? a->workspace : nullptr, bg_train_step_depth_workspace_bytes(n, k, w, h), w, h);
+    if (int32_t r = check_workspace_bytes(who, bl ? "bg_train_step_bilagrid_workspace_bytes" : d ? "bg_train_step_depth_workspace_bytes"
+                                                                                             : "bg_train_step_workspace_bytes",
+                                          a->workspace_bytes, bl ? bws.bytes : d ? dws.bytes : ws.bytes); r != BG_OK) return r;
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
     int32_t r;
@@ -835,7 +881,10 @@ static int32_t train_step(BgContext *c, void *stream, BgTrainStepArgs *a, const 
                        ws.out_img, dws.depth, ws.visible, ws.max_radius, &a->state_out);
     if (r != BG_OK) return r;
     BG_CUDA(cudaMemsetAsync(ws.v_output, 0, (size_t)w * h * 4 * sizeof(float), s));
-    if ((r = view_loss(c, stream, a, a->gt_packed, ws, a->loss_out, d, dws)) != BG_OK) return r;
+    if (bl) BG_CUDA(launch_bilagrid_slice(s, bl->grid, ws.out_img, w, h, bws.sliced));
+    if ((r = view_loss(c, stream, a, a->gt_packed, ws, bl ? bws.sliced : ws.out_img, a->loss_out, d, dws)) != BG_OK) return r;
+    // the gradient w.r.t. the sliced image back to the raw one, in place; the blend backward replays the RAW out_img
+    if (bl) BG_CUDA(launch_bilagrid_slice_bwd(s, bl->grid, ws.out_img, ws.v_output, w, h, ws.v_output, bws.v_grid));
     // backward (bwd/burn_glue.rs:121-182); the depth gradient reaches the means through v_z
     r = rasterize_backward(c, stream, &a->state_out, ws.out_img, dws.depth, ws.v_output, dws.v_depth, a->background, 0, ws.v_combined,
                            n, dws.v_z, d ? "bg_rasterize_backward_depth" : "bg_rasterize_backward");
@@ -845,17 +894,19 @@ static int32_t train_step(BgContext *c, void *stream, BgTrainStepArgs *a, const 
     if (r != BG_OK) return r;
     if (d) BG_CUDA(launch_depth_to_means(s, a->state_out.compact_from_global_gid, dws.v_z, a->state_out.n, a->cam, ws.v_t));
     // optimiser, refine statistics, mean noise (train.rs:280-416): one pass over the Gaussians, as bg_train_update
-    if (n == 0) return BG_OK;
-    UpdateParams P = update_params(a);
-    P.g_t = ws.v_t; P.g_o = ws.v_o; P.g_sh = ws.v_sh;
-    P.v_refine = ws.v_r; P.max_radius = ws.max_radius; P.visible = ws.visible;
-    BG_CUDA(launch_train_update(s, sh_degree_from_k(k), P, false));
+    if (n > 0) {
+        UpdateParams P = update_params(a);
+        P.g_t = ws.v_t; P.g_o = ws.v_o; P.g_sh = ws.v_sh;
+        P.v_refine = ws.v_r; P.max_radius = ws.max_radius; P.visible = ws.visible;
+        BG_CUDA(launch_train_update(s, sh_degree_from_k(k), P, false));
+    }
+    if (bl) BG_CUDA(bilagrid_update(s, bl, bws.v_grid, a->loss_out));
     return BG_OK;
 }
 
 extern "C" int32_t bg_train_step(BgContext *c, void *stream, BgTrainStepArgs *a) {
     if (!c || !a) return BG_ERR_NULL;
-    return train_step(c, stream, a, nullptr);
+    return train_step(c, stream, a, nullptr, nullptr);
 }
 
 // ---- bg_train_step_depth: bg_train_step with the depth-supervision term of DESIGN.md section 4.7
@@ -864,12 +915,67 @@ extern "C" int32_t bg_train_step_depth(BgContext *c, void *stream, BgTrainStepAr
     if (int32_t r = check_depth(*d, "bg_train_step_depth"); r != BG_OK) return r;
     if (!depth_term(*d)) {
         // no term (target may be null): the plain step, launch for launch, and a zero depth loss
-        const int32_t r = train_step(c, stream, a, nullptr);
+        const int32_t r = train_step(c, stream, a, nullptr, nullptr);
         if (r != BG_OK) return r;
         BG_CUDA(cudaMemsetAsync(d->depth_loss_out, 0, sizeof(float), (cudaStream_t)stream));
         return BG_OK;
     }
-    return train_step(c, stream, a, d);
+    return train_step(c, stream, a, d, nullptr);
+}
+
+// ---- the bilateral grid of DESIGN.md section 4.11
+extern "C" int32_t bg_bilagrid_slice(BgContext *c, void *stream, const float *grid, const float *img, uint32_t h, uint32_t w,
+                                     float *out) {
+    if (!c || !grid || !img || !out) return BG_ERR_NULL;
+    if (!aligned16(grid) || !aligned16(img) || !aligned16(out))
+        return invalid("bg_bilagrid_slice", "grid, img and out must be 16-byte aligned");
+    if (h == 0 || w == 0) return BG_OK;
+    if (overlap(img, out, h, w)) return invalid("bg_bilagrid_slice", "out must not overlap img");
+    BG_CUDA(cudaSetDevice(c->device));
+    BG_CUDA(launch_bilagrid_slice((cudaStream_t)stream, grid, img, w, h, out));
+    return BG_OK;
+}
+
+extern "C" int32_t bg_bilagrid_slice_backward(BgContext *c, void *stream, const float *grid, const float *img, const float *v_out,
+                                              uint32_t h, uint32_t w, float *v_img, float *v_grid) {
+    if (!c || !grid || !img || !v_out || !v_img || !v_grid) return BG_ERR_NULL;
+    if (!aligned16(grid) || !aligned16(img) || !aligned16(v_out) || !aligned16(v_img) || !aligned16(v_grid))
+        return invalid("bg_bilagrid_slice_backward", "grid, img, v_out, v_img and v_grid must be 16-byte aligned");
+    if (overlap(img, v_img, h, w) || (v_img != v_out && overlap(v_out, v_img, h, w)))
+        return invalid("bg_bilagrid_slice_backward", "v_img must not overlap img, and must be v_out itself or not overlap it");
+    BG_CUDA(cudaSetDevice(c->device));
+    if (h == 0 || w == 0) {
+        BG_CUDA(cudaMemsetAsync(v_grid, 0, sizeof(float) * BG_BILAGRID_FLOATS, (cudaStream_t)stream));
+        return BG_OK;
+    }
+    BG_CUDA(launch_bilagrid_slice_bwd((cudaStream_t)stream, grid, img, v_out, w, h, v_img, v_grid));
+    return BG_OK;
+}
+
+extern "C" int32_t bg_bilagrid_update(BgContext *c, void *stream, const BgBilagridStep *b, float *v_grid) {
+    if (!c || !v_grid) return BG_ERR_NULL;
+    if (int32_t r = check_bilagrid_step(b, "bg_bilagrid_update"); r != BG_OK) return r;
+    if (!aligned16(v_grid)) return invalid("bg_bilagrid_update", "v_grid must be 16-byte aligned");
+    BG_CUDA(cudaSetDevice(c->device));
+    BG_CUDA(bilagrid_update((cudaStream_t)stream, b, v_grid, nullptr));
+    return BG_OK;
+}
+
+// ---- bg_train_step_bilagrid: the single-view step with the view's bilateral grid, with or without the depth term
+extern "C" int32_t bg_train_step_bilagrid(BgContext *c, void *stream, BgTrainStepArgs *a, const BgDepthSupervision *d,
+                                          const BgBilagridStep *bl) {
+    if (!c || !a || !bl) return BG_ERR_NULL;
+    if (int32_t r = check_bilagrid_step(bl, "bg_train_step_bilagrid"); r != BG_OK) return r;
+    if (d) {
+        if (int32_t r = check_depth(*d, "bg_train_step_bilagrid"); r != BG_OK) return r;
+        if (!depth_term(*d)) {
+            const int32_t r = train_step(c, stream, a, nullptr, bl);
+            if (r != BG_OK) return r;
+            BG_CUDA(cudaMemsetAsync(d->depth_loss_out, 0, sizeof(float), (cudaStream_t)stream));
+            return BG_OK;
+        }
+    }
+    return train_step(c, stream, a, d, bl);
 }
 
 // ---- view-sharded data parallelism (dp.cu): communicator, exchange, the multi-view step
@@ -1090,7 +1196,7 @@ static int32_t train_step_views(BgContext *c, BgDpComm *h, void *stream, BgTrain
         r = render_forward(c, stream, cam, w, hh, n, k, r_t, a->sh, r_o, a->mip, a->background, BG_PASS_BACKWARD, ws.out_img, vd.depth,
                            ws.visible, ws.max_radius, &a->state_out);
         if (r != BG_OK) return r;
-        if ((r = view_loss(c, stream, a, a->gt_packed[i], ws, ws.loss_terms + i, di, dws)) != BG_OK) return r;
+        if ((r = view_loss(c, stream, a, a->gt_packed[i], ws, ws.out_img, ws.loss_terms + i, di, dws)) != BG_OK) return r;
         r = rasterize_backward(c, stream, &a->state_out, ws.out_img, vd.depth, ws.v_output, vd.v_depth, a->background, 0, ws.v_combined, n,
                                vd.v_z, di ? "bg_rasterize_backward_depth" : "bg_rasterize_backward");
         if (r != BG_OK) return r;

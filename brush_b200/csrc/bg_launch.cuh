@@ -225,4 +225,13 @@ cudaError_t launch_depth_loss_fused(cudaStream_t s, const float *out_img, const 
 cudaError_t launch_depth_loss_reduce(cudaStream_t s, const float *partials, uint32_t count, float chain, float *depth_loss_out,
                                      float *loss_out);
 
+// ---- bilagrid.cu
+// grid [L,H,W,12], img / out float4 [h,w] (out may not alias img)
+cudaError_t launch_bilagrid_slice(cudaStream_t s, const float *grid, const float *img, uint32_t w, uint32_t h, float *out);
+// v_img = the adjoint of the slice w.r.t. img (may alias v_out); v_grid [L,H,W,12] is overwritten
+cudaError_t launch_bilagrid_slice_bwd(cudaStream_t s, const float *grid, const float *img, const float *v_out, uint32_t w,
+                                      uint32_t h, float *v_img, float *v_grid);
+// v_grid += tv_weight * dTV/dgrid; *tv_out = tv_weight * TV(grid); *loss_out (may be null) += the same
+cudaError_t launch_bilagrid_tv(cudaStream_t s, const float *grid, float *v_grid, float tv_weight, float *tv_out, float *loss_out);
+
 }  // namespace bg

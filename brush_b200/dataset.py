@@ -864,7 +864,8 @@ class SceneLoader:
             t = t.pin_memory()      # cached batches are uploaded many times: pin them once
             depth = depth.pin_memory() if depth is not None else None
         batch = SceneBatch(img_packed=t, camera=v.camera, has_alpha=has_alpha,
-                           masked_alpha=has_alpha and self.alpha_mode == ALPHA_MASKED, depth=depth, depth_count=depth_count)
+                           masked_alpha=has_alpha and self.alpha_mode == ALPHA_MASKED, depth=depth, depth_count=depth_count,
+                           view_index=index)
         if admit:
             with self._lock:
                 if self._cache[index] is not None:

@@ -25,6 +25,8 @@ class EvalSample:
     depth_abs_rel: Optional[torch.Tensor] = None    # mean |ed - t| / t over the active pixels (ed = D / alpha)
     depth_rmse: Optional[torch.Tensor] = None       # sqrt(mean (ed - t)^2) over the active pixels, scene units
     depth_coverage: Optional[torch.Tensor] = None   # |active| / |valid|
+    cc_psnr: Optional[torch.Tensor] = None          # PSNR / SSIM after the affine colour correction (colour_correct=True)
+    cc_ssim: Optional[torch.Tensor] = None
 
     def save_to_disk(self, path: str) -> None:
         """eval.rs:66-81: the rendered image (already on the 8-bit grid) as an 8-bit RGB file; parent directories are
@@ -37,12 +39,14 @@ class EvalSample:
 
 
 def eval_stats(ctx: RenderContext, splats, camera, gt_image: np.ndarray, alpha_mode: str = ALPHA_MASKED,
-               render_mip: bool = False, gt_depth: Optional[np.ndarray] = None) -> EvalSample:
+               render_mip: bool = False, gt_depth: Optional[np.ndarray] = None, colour_correct: bool = False) -> EvalSample:
     """splats: train.Splats (a min-scale floor is folded in, as in render_splats, gaussian_splats.rs:379-384).
     render_mip: the splats' render mode -- evaluation renders with the filter the model is trained with
     (gaussian_splats.rs:395: `splats.render_mip`).  gt_image: [H,W,3] or [H,W,4] u8; an alpha channel goes through
     view_to_packed_data(alpha_mode) like a training view (eval.rs:31).  gt_depth: optional f32 [H,W] depth target
-    (SceneView.load_depth); adds the depth metrics, which are NaN when no pixel is active."""
+    (SceneView.load_depth); adds the depth metrics, which are NaN when no pixel is active.  colour_correct adds cc_psnr
+    and cc_ssim (affine_colour_correct).  This is an affine least-squares fit, not MultiNeRF's iterative quadratic
+    colour correction, so these numbers are not gsplat's cc_psnr."""
     h, w = gt_image.shape[0], gt_image.shape[1]
     packed, _ = view_to_packed_data(gt_image, alpha_mode)
     gt = torch.from_numpy(packed).to(ctx.device)
@@ -56,6 +60,12 @@ def eval_stats(ctx: RenderContext, splats, camera, gt_image: np.ndarray, alpha_m
     psnr = torch.log(1.0 / mse) * 10.0 / float(np.log(10.0))
     ssim = image_loss_forward(ctx, rgb, gt, 3, ImageLossConfig(0.0, 1.0, None, False)).mean()
     sample = EvalSample(rendered=rgb, psnr=psnr, ssim=ssim, render_aux=out)
+    if colour_correct:
+        gt_rgb = gt.view(torch.uint8).reshape(h, w, 4)[..., 0:3].double() / 255.0
+        cc = affine_colour_correct(rgb, gt_rgb)
+        sample.cc_psnr = torch.log(1.0 / image_loss_forward(ctx, cc, gt, 3, ImageLossConfig(1.0, 0.0, None, False)).pow(2).mean()) \
+            * 10.0 / float(np.log(10.0))
+        sample.cc_ssim = image_loss_forward(ctx, cc, gt, 3, ImageLossConfig(0.0, 1.0, None, False)).mean()
     if gt_depth is not None:
         if tuple(gt_depth.shape) != (h, w):
             raise ValueError(f"gt_depth must be [{h},{w}], got {tuple(gt_depth.shape)}")
@@ -72,3 +82,14 @@ def eval_stats(ctx: RenderContext, splats, camera, gt_image: np.ndarray, alpha_m
         nv = valid.sum()
         sample.depth_coverage = cnt.double() / nv.double() if bool(nv > 0) else nan
     return sample
+
+
+def affine_colour_correct(rgb: torch.Tensor, gt_rgb: torch.Tensor) -> torch.Tensor:
+    """rgb [h,w,3] (the 8-bit render) mapped by the float64 least-squares 3x4 affine A minimising |A [rgb; 1] - gt|^2
+    over all pixels, clamped to [0, 1] and rounded to 8 bit; float32 [h,w,3].  An affine fit, not MultiNeRF's
+    iterative quadratic colour correction."""
+    x = rgb.reshape(-1, 3).double()
+    x = torch.cat([x, torch.ones_like(x[:, :1])], dim=1)
+    a = torch.linalg.lstsq(x.cpu(), gt_rgb.reshape(-1, 3).double().cpu()).solution.to(x.device)
+    cc = (x @ a).clamp(0.0, 1.0).reshape(rgb.shape)
+    return (torch.round(cc * 255.0) / 255.0).float().contiguous()

@@ -115,7 +115,13 @@ def train_loop(ctx, splats, train_views: Sequence, eval_views: Sequence, config,
     process = process or ProcessConfig()
     from PIL import Image
     loader = SceneLoader(train_views, alpha_mode, seed=process.seed)
-    trainer = SplatTrainer(config, ctx, bounds_from_pos_device(ctx, BOUND_PERCENTILE, splats.transforms))
+    # one grid per training view (DESIGN.md section 4.11), shared by every LOD level's trainer: its coordinates are
+    # normalised, so it stays valid on the downscaled images
+    grids = None
+    if config.bilateral_grid:
+        from .bilagrid import BilateralGrids
+        grids = BilateralGrids(len(train_views), splats.transforms.device)
+    trainer = SplatTrainer(config, ctx, bounds_from_pos_device(ctx, BOUND_PERCENTILE, splats.transforms), bilateral_grids=grids)
     # refine grows the model up to config.max_splats: the context must have been created for it (the reference sizes
     # its buffers per render; here capacity is fixed at bg_ctx_create)
     cap = min(int(config.max_splats), max(int(ctx.max_splats), 0))
@@ -173,7 +179,8 @@ def train_loop(ctx, splats, train_views: Sequence, eval_views: Sequence, config,
             splats.transforms, splats.sh_coeffs, splats.raw_opacities, splats.min_scale = (
                 kept.transforms, kept.sh_coeffs, kept.raw_opacities, kept.min_scale)
             level = target
-            trainer = SplatTrainer(config, ctx, bounds_from_pos_device(ctx, BOUND_PERCENTILE, splats.transforms))
+            trainer = SplatTrainer(config, ctx, bounds_from_pos_device(ctx, BOUND_PERCENTILE, splats.transforms),
+                                   bilateral_grids=grids)
             trainer.set_view_cams(view_cams)
             if config.lod_image_scale < 100:               # a rebuild at 100 % would only drop the warm batch cache
                 loader.close()
@@ -192,17 +199,23 @@ def train_loop(ctx, splats, train_views: Sequence, eval_views: Sequence, config,
             on_step(done, stats, refine)
         if eval_views and should_eval_lod(done, level, process.eval_every, total):
             check_overflow()
-            psnr, ssim, dm = [], [], []
+            psnr, ssim, dm, cc = [], [], [], []
             for v in eval_views:
                 gt = v.load_image()                        # view.image.load(): a mask file, if any, is the alpha channel
                 gt_depth = v.load_depth() if v.depth_path is not None else None
-                s = eval_stats(ctx, splats, v.camera, gt, alpha_mode, render_mip=config.render_mip, gt_depth=gt_depth)
+                # the raw model: held-out views have no grid.  With grids, also the colour-corrected metrics
+                s = eval_stats(ctx, splats, v.camera, gt, alpha_mode, render_mip=config.render_mip, gt_depth=gt_depth,
+                               colour_correct=grids is not None)
                 psnr.append(float(s.psnr)); ssim.append(float(s.ssim))
+                if grids is not None:
+                    cc.append((float(s.cc_psnr), float(s.cc_ssim)))
                 if gt_depth is not None:
                     dm.append((float(s.depth_abs_rel), float(s.depth_rmse), float(s.depth_coverage)))
                 if process.eval_save_to_disk:              # train_stream.rs:543-550
                     s.save_to_disk(os.path.join(process.export_path, f"eval_{done}", f"{v.img_name()}.png"))
             rec = {"iter": done, "psnr": float(np.mean(psnr)), "ssim": float(np.mean(ssim)), "splats": splats.num_splats()}
+            if cc:
+                rec["cc_psnr"], rec["cc_ssim"] = (float(np.mean(col)) for col in np.array(cc, np.float64).T)
             if dm:                                         # only when the eval views carry depth (means over those views)
                 for key, col in zip(("depth_abs_rel", "depth_rmse", "depth_coverage"), np.array(dm, np.float64).T):
                     rec[key] = float(np.mean(col))

@@ -21,6 +21,9 @@ provides memory, streams and (for N>1) torch.distributed.
                          into scales/opacity for every render, its gradient chained back in place, baked at the
                          start of refine() and recomputed at its end while progress < 0.9 (train.rs:437, 641-647).
 
+  bilateral_grids       <- per-view appearance compensation (DESIGN.md section 4.11): step() and step_fused() slice the
+                         render by the view's grid before the loss and update that grid after the splats (bilagrid.py)
+
 Out of scope here: LPIPS.
 """
 from __future__ import annotations
@@ -34,6 +37,8 @@ import numpy as np
 import torch
 
 from . import _lib
+from . import bilagrid as _bilagrid
+from .bilagrid import BilateralGrids, bilagrid_lr
 from .camera import Camera
 from .loss import ImageLossConfig, depth_loss_fused, image_loss_fused
 from .render import (PASS_BACKWARD, RenderContext, _stream_ptr, project_bwd, project_bwd_factored, rasterize_bwd,
@@ -67,6 +72,11 @@ class TrainConfig:
     # map; 0 leaves the step exactly as without it.  Keyword-only, so the positional order of every other field and the
     # trailing seed + LOD fields stay as they were.
     depth_loss_weight: float = field(default=0.0, kw_only=True)
+    # per-view appearance compensation (DESIGN.md section 4.11): a bilateral grid per training view, learned with the
+    # splats at bilagrid_lr(bilateral_grid_lr, n, total_train_iters) under a TV regulariser of this weight
+    bilateral_grid: bool = field(default=False, kw_only=True)
+    bilateral_grid_lr: float = field(default=2e-3, kw_only=True)
+    bilateral_grid_tv_weight: float = field(default=10.0, kw_only=True)
     seed: int = 0  # the reference uses an unseeded rand::rng(); a shared seed keeps DP ranks identical
     # LOD baking (config.rs:108-125): after the main run, lod_levels times score, keep lod_decimation_keep % of the splats
     # and retrain lod_refine_steps steps on images scaled by lod_image_scale % per level
@@ -78,6 +88,12 @@ class TrainConfig:
     def __post_init__(self):
         if not (math.isfinite(self.depth_loss_weight) and self.depth_loss_weight >= 0.0):
             raise ValueError(f"depth_loss_weight must be finite and >= 0, got {self.depth_loss_weight}")
+        if not isinstance(self.bilateral_grid, bool):
+            raise ValueError(f"bilateral_grid must be a bool, got {self.bilateral_grid!r}")
+        for name in ("bilateral_grid_lr", "bilateral_grid_tv_weight"):
+            v = getattr(self, name)
+            if not (isinstance(v, (int, float)) and math.isfinite(v) and v >= 0.0):
+                raise ValueError(f"{name} must be finite and >= 0, got {v!r}")
         if self.lod_levels < 0:
             raise ValueError("lod_levels must be >= 0")
         for name in ("lod_decimation_keep", "lod_image_scale"):
@@ -151,6 +167,7 @@ class SceneBatch:
     masked_alpha: bool = False    # AlphaMode::Masked
     depth: Optional[torch.Tensor] = None   # [H,W] f32 metric camera-space z target, 0 = no measurement; host (pinned) or device
     depth_count: int = 0                    # valid pixels of `depth` (finite and > 0), counted on the host
+    view_index: int = -1                    # position of the view in the training views (selects its bilateral grid)
 
     def img_size(self):
         return int(self.img_packed.shape[0]), int(self.img_packed.shape[1])
@@ -231,12 +248,21 @@ class TrainStepStats:
     loss: torch.Tensor  # lazy device scalar (msg.rs:16-27); image loss + depth loss
     depth_loss: Optional[torch.Tensor] = None   # the depth term alone (None when the batch carries no depth)
     view_depth_losses: Optional[torch.Tensor] = None   # step_views_depth: device [local views], each view's depth term
+    # with bilateral grids: the TV term of the view's grid (included in loss).  step() hands out a copy; step_fused() a
+    # view of the grids' buffer that the next step overwrites, as its loss
+    tv_loss: Optional[torch.Tensor] = None
 
 
 class SplatTrainer:
     def __init__(self, config: TrainConfig, ctx: RenderContext, bounds: BoundingBox,
-                 grad_hook: Optional[Callable[[Sequence[torch.Tensor]], None]] = None):
+                 grad_hook: Optional[Callable[[Sequence[torch.Tensor]], None]] = None,
+                 bilateral_grids: Optional[BilateralGrids] = None):
         self.config = config
+        # the views' grids (DESIGN.md section 4.11): present exactly when config.bilateral_grid asks for them
+        if config.bilateral_grid != (bilateral_grids is not None):
+            raise ValueError("TrainConfig.bilateral_grid needs SplatTrainer(..., bilateral_grids=BilateralGrids(views, device)), "
+                             "and grids need bilateral_grid=True")
+        self.bilateral_grids = bilateral_grids
         self.ctx = ctx
         self.bounds = bounds
         self.lr_mean_decay = (config.lr_mean_end / config.lr_mean) ** (1.0 / config.total_train_iters)
@@ -261,6 +287,7 @@ class SplatTrainer:
         self._fused_loss = None
         self._fused_depth_loss = None
         self._v_output_depth = None
+        self._sliced = None
 
     def set_view_cams(self, view_cams) -> None:
         """train.rs:172-174.  view_cams: sequence of ((x, y, z), focal_px) of the training views."""
@@ -347,6 +374,8 @@ class SplatTrainer:
         background = self.sample_background()
         median_scale = self.bounds.median_size()
 
+        grids = self.bilateral_grids
+        view = grids.check_view(batch.view_index) if grids is not None else None
         r_transforms, r_raw_opac = splats.folded(self.ctx)   # 3D-filter floor folded in (bwd/burn_glue.rs:260-270)
         out = render_splats(self.ctx, batch.camera, (img_w, img_h), r_transforms, splats.sh_coeffs,
                             r_raw_opac, mip=cfg.render_mip, background=background, rpass=PASS_BACKWARD, render_depth=depth)
@@ -364,10 +393,18 @@ class SplatTrainer:
                 self._v_output = torch.zeros_like(out.out_img)   # channel 3 stays zero unless alpha matching
                 self._v_output_ch = channels
             v_output = self._v_output
+        loss_img = out.out_img
+        if grids is not None:   # the loss sees the render through the view's grid
+            if self._sliced is None or self._sliced.shape != out.out_img.shape:
+                self._sliced = torch.empty_like(out.out_img)
+            loss_img = _bilagrid.slice(self.ctx, grids.grids[view], out.out_img, out=self._sliced)
         # value and gradient of the loss from the fused kernel in one pass
-        v_output, loss = image_loss_fused(self.ctx, out.out_img, gt_packed, channels, lcfg, chain, v_output)
+        v_output, loss = image_loss_fused(self.ctx, loss_img, gt_packed, channels, lcfg, chain, v_output)
         if depth:
             v_depth, depth_loss = depth_loss_fused(self.ctx, out.out_img, out.depth, target, self._depth_chain(batch), v_output)
+        if grids is not None:   # back through the slice, in place; the blend backward replays the RAW render
+            _bilagrid.slice_backward(self.ctx, grids.grids[view], out.out_img, v_output, v_img=v_output, v_grid=grids.v_grid)
+        if depth:
             v_combined, v_z = rasterize_bwd_depth(out, v_output, v_depth)
         else:
             v_combined, v_z = rasterize_bwd(out, v_output), None
@@ -378,16 +415,28 @@ class SplatTrainer:
             self.grad_hook((v_t, v_sh, v_o, v_r, out.visible, out.max_radius))
 
         lr_mean = self._apply_updates(splats, v_t, v_sh, v_o, v_r, out.visible, out.max_radius, median_scale)
+        tv = None
+        if grids is not None:
+            tv = _bilagrid.update(self.ctx, grids, view, grids.v_grid, self._bilagrid_lr(), cfg.bilateral_grid_tv_weight).clone()
         if depth:
-            return TrainStepStats(num_visible_event=out, lr_mean=lr_mean, loss=loss + depth_loss, depth_loss=depth_loss)
+            total = loss + depth_loss
+            return TrainStepStats(num_visible_event=out, lr_mean=lr_mean, loss=total if tv is None else total + tv,
+                                  depth_loss=depth_loss, tv_loss=tv)
         depth_loss = torch.zeros((), dtype=torch.float32, device=dev) if batch.depth is not None else None
-        return TrainStepStats(num_visible_event=out, lr_mean=lr_mean, loss=loss, depth_loss=depth_loss)
+        return TrainStepStats(num_visible_event=out, lr_mean=lr_mean, loss=loss if tv is None else loss + tv,
+                              depth_loss=depth_loss, tv_loss=tv)
+
+    def _bilagrid_lr(self) -> float:
+        """The grids' learning rate of the current step_count, in f32."""
+        cfg = self.config
+        return float(np.float32(bilagrid_lr(cfg.bilateral_grid_lr, self.step_count, cfg.total_train_iters)))
 
     # ------------------------------------------------------------------------------------------------
     def step_fused(self, batch: SceneBatch, splats: Splats) -> TrainStepStats:
         """The same step through ONE ABI call (bg_train_step): every launch of the step is issued by the library on
         the current stream, scratch comes from a workspace allocated once.  No min-scale floor, no gradient hook.
-        A batch that carries depth goes through bg_train_step_depth (the depth term of DESIGN.md section 4.7)."""
+        A batch that carries depth goes through bg_train_step_depth (the depth term of DESIGN.md section 4.7); with
+        bilateral grids the step is bg_train_step_bilagrid, with or without the depth term."""
         if splats.min_scale is not None or self.grad_hook is not None:
             raise ValueError("step_fused handles the plain single-view step; use step() with a scale floor or a gradient hook")
         cfg = self.config
@@ -401,12 +450,18 @@ class SplatTrainer:
         median_scale = self.bounds.median_size()
         n, k = splats.num_splats(), splats.sh_coeffs.shape[1]
         with_depth = batch.depth is not None
-        need = int((lib.bg_train_step_depth_workspace_bytes if with_depth else lib.bg_train_step_workspace_bytes)(n, k, img_w, img_h))
+        grids = self.bilateral_grids
+        view = grids.check_view(batch.view_index) if grids is not None else None
+        sizer = (lib.bg_train_step_bilagrid_workspace_bytes if grids is not None else
+                 lib.bg_train_step_depth_workspace_bytes if with_depth else lib.bg_train_step_workspace_bytes)
+        need = int(sizer(n, k, img_w, img_h))
         if self._fused_ws is None or self._fused_ws.numel() < need:
             self._fused_ws = torch.empty(need, dtype=torch.uint8, device=dev)
             self._fused_loss = torch.zeros(1, dtype=torch.float32, device=dev)
         a, lr_mean = self._fused_args(batch, splats, gt_packed, background, median_scale, self._fused_ws, need)
         a.loss_out = self._fused_loss.data_ptr()
+        if grids is not None:
+            return self._step_fused_bilagrid(batch, a, lr_mean, view, with_depth)
         if not with_depth:
             _lib.check(lib.bg_train_step(self.ctx.handle, _stream_ptr(dev), C.byref(a)), "bg_train_step")
             return TrainStepStats(num_visible_event=None, lr_mean=lr_mean, loss=self._fused_loss[0])
@@ -422,6 +477,25 @@ class SplatTrainer:
         self._fused_keepalive = target
         return TrainStepStats(num_visible_event=None, lr_mean=lr_mean, loss=self._fused_loss[0],
                               depth_loss=self._fused_depth_loss[0])
+
+    def _step_fused_bilagrid(self, batch: SceneBatch, a, lr_mean: float, view: int, with_depth: bool) -> TrainStepStats:
+        cfg, dev, lib = self.config, self.ctx.device, _lib.load()
+        grids = self.bilateral_grids
+        ds, target = None, None
+        if with_depth:
+            if self._fused_depth_loss is None:
+                self._fused_depth_loss = torch.zeros(1, dtype=torch.float32, device=dev)
+            ds = _lib.BgDepthSupervision()
+            target = self._depth_target(batch) if self._depth_term(batch) else None
+            ds.target = target.data_ptr() if target is not None else None
+            ds.weight, ds.valid_count = float(cfg.depth_loss_weight), int(batch.depth_count)
+            ds.depth_loss_out = self._fused_depth_loss.data_ptr()
+        bl = grids.step_args(view, self._bilagrid_lr(), cfg.bilateral_grid_tv_weight)
+        _lib.check(lib.bg_train_step_bilagrid(self.ctx.handle, _stream_ptr(dev), C.byref(a), C.byref(ds) if ds is not None else None,
+                                              C.byref(bl)), "bg_train_step_bilagrid")
+        self._fused_keepalive = target
+        return TrainStepStats(num_visible_event=None, lr_mean=lr_mean, loss=self._fused_loss[0],
+                              depth_loss=self._fused_depth_loss[0] if with_depth else None, tv_loss=grids.tv_loss[0])
 
     def _fused_args(self, batch: SceneBatch, splats: Splats, gt_packed, background, median_scale, ws, need):
         """BgTrainStepArgs of step_fused for the current step_count (loss_out left unset)."""
@@ -476,6 +550,8 @@ class SplatTrainer:
     def _step_views(self, batches, splats, group, chunks, distributed, with_depth: bool) -> TrainStepStats:
         import torch.distributed as dist
         cfg = self.config
+        if self.bilateral_grids is not None:
+            raise ValueError("step_views and step_views_depth do not train bilateral grids: use step() or step_fused()")
         self._ensure_state(splats)
         dev = self.ctx.device
         lib = _lib.load()

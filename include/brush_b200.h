@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define BG_ABI_VERSION 11u
+#define BG_ABI_VERSION 12u
 
 /* f32 lanes per projected splat: a 64-byte row, four aligned 128-bit loads.  Lanes 0..8 are the reference
  * layout (kernels/helpers.rs:49-53: xy_x, xy_y, conic_x, conic_y, conic_z, color_a, color_r, color_g, color_b).
@@ -482,6 +482,48 @@ int32_t bg_sparse_mesh_count(BgContext *ctx, void *stream, const BgSparseTsdfGri
                              uint64_t workspace_bytes, uint32_t *num_vertices /* host */, uint32_t *num_triangles /* host */);
 int32_t bg_sparse_mesh_emit(BgContext *ctx, void *stream, const BgSparseTsdfGrid *grid, void *workspace, uint64_t workspace_bytes,
                             uint32_t max_vertices, uint32_t max_triangles, float *vertices, uint8_t *colors, uint32_t *faces);
+
+/* ---- Per-view appearance compensation (DESIGN.md section 4.11; Wang et al., SIGGRAPH 2024): each training view owns a
+ * bilateral grid of 3x4 affine colour transforms A = [M | b], f32, cell-major [L][H][W][12] (z, y, x, row-major A),
+ * 16-byte aligned, identity (M = I, b = 0) at the start.
+ * bg_bilagrid_slice: out [h,w,4] = (M c + b, a) for img [h,w,4] = (c, a), A trilinear at
+ *   ((px + 0.5) / w * (W-1), (py + 0.5) / h * (H-1), clamp(0.299 c_r + 0.587 c_g + 0.114 c_b, 0, 1) * (L-1))
+ *   (grid_sample, bilinear, border padding, align_corners).  out must not overlap img (else BG_ERR_INVALID).
+ * bg_bilagrid_slice_backward: from v_out [h,w,4] = dL/dout, writes v_img = dL/dimg (the luminance guidance included where
+ *   0 < gray < 1; alpha passes through) and OVERWRITES v_grid [L,H,W,12] with dL/dgrid.  v_img may be v_out itself (in
+ *   place); it must not overlap img, nor overlap v_out in any other way (else BG_ERR_INVALID).  v_grid must not overlap
+ *   the images or the grid.
+ * bg_bilagrid_update: v_grid (the gradient from bg_bilagrid_slice_backward; BgBilagridStep names only the state it
+ *   updates) += tv_weight * dTV/dgrid, *tv_loss_out = tv_weight * TV(grid) with
+ *   TV(G) = sum over the axes of (1/P_axis) * the sum of squared neighbour differences (P_axis: their count), then one
+ *   Adam step (betas 0.9, 0.999, eps 1e-15, 1-based step: the view's own count) on (grid, v_grid, m, v).
+ * img, out, v_out, v_img, grid, v_grid, m and v: 16-byte aligned, else BG_ERR_INVALID; step < 1 or a negative or
+ * non-finite lr or tv_weight is BG_ERR_INVALID; null pointers are BG_ERR_NULL.  Checked before any launch. */
+#define BG_BILAGRID_L 8
+#define BG_BILAGRID_H 16
+#define BG_BILAGRID_W 16
+#define BG_BILAGRID_FLOATS (BG_BILAGRID_L * BG_BILAGRID_H * BG_BILAGRID_W * 12)
+typedef struct {
+    float *grid, *m, *v;      /* device [L,H,W,12] each: the view's grid and its Adam moments, updated in place */
+    int32_t step;             /* the view's 1-based Adam step */
+    float lr, tv_weight;      /* the step's learning rate (the caller evaluates the schedule), the TV weight */
+    float *tv_loss_out;       /* device scalar: tv_weight * TV(grid) before the update */
+} BgBilagridStep;
+int32_t bg_bilagrid_slice(BgContext *ctx, void *stream, const float *grid, const float *img /*[h,w,4]*/, uint32_t h, uint32_t w,
+                          float *out /*[h,w,4]*/);
+int32_t bg_bilagrid_slice_backward(BgContext *ctx, void *stream, const float *grid, const float *img, const float *v_out,
+                                   uint32_t h, uint32_t w, float *v_img, float *v_grid);
+int32_t bg_bilagrid_update(BgContext *ctx, void *stream, const BgBilagridStep *step, float *v_grid /* += the TV gradient */);
+
+/* bg_train_step (or bg_train_step_depth when depth is non-null) with the view's grid between the render and the loss:
+ * the image loss is taken on bg_bilagrid_slice of the raw render, its gradient goes back through
+ * bg_bilagrid_slice_backward to the raw render (which the blend backward replays), and bg_bilagrid_update runs on the
+ * grid after the splat update.  The depth term reads the raw alpha and depth.  *args->loss_out = image loss (+ L_d) +
+ * L_tv.  Nothing is read back (capturable in a CUDA graph).  workspace: bg_train_step_bilagrid_workspace_bytes(n, k, w, h)
+ * bytes (else BG_ERR_CAPACITY).  Every check of bg_train_step, bg_train_step_depth and bg_bilagrid_update applies. */
+uint64_t bg_train_step_bilagrid_workspace_bytes(uint32_t n, uint32_t k, uint32_t w, uint32_t h);
+int32_t bg_train_step_bilagrid(BgContext *ctx, void *stream, BgTrainStepArgs *args, const BgDepthSupervision *depth /* nullable */,
+                               const BgBilagridStep *bilagrid);
 
 /* ---- View-sharded data parallelism behind the boundary (SURVEY.md section 8e; the reference is single-device).
  * A communicator is one NCCL rank bound to the context's device.  Rank 0 calls bg_dp_unique_id and ships the 128 bytes

@@ -446,6 +446,56 @@ struct TrainConfig {                         // brush-train/src/config.rs:5-132 
     float split_at_screen_size = 0.5f;
     // depth supervision (DESIGN.md section 4.7): weight of the L1 term on the expected depth; 0 = the plain step
     float depth_loss_weight = 0.0f;
+    // per-view appearance compensation (DESIGN.md section 4.11): the grids' base learning rate (bilagrid_lr) and TV weight.
+    // SplatTrainer's grid step overload requires bilateral_grid; the other steps refuse it.
+    bool bilateral_grid = false;
+    double bilateral_grid_lr = 2e-3;
+    float bilateral_grid_tv_weight = 10.0f;
+};
+
+// lr(n) = lr0 (0.01 + 0.99 min(n - 1, 1000) / 1000) 0.01^((n - 1) / total_train_iters), n 1-based (DESIGN.md section 4.11)
+inline double bilagrid_lr(double lr0, int n, uint32_t total_train_iters) {
+    return lr0 * (0.01 + 0.99 * (double)std::min(n - 1, 1000) / 1000.0) * std::pow(0.01, (double)(n - 1) / (double)total_train_iters);
+}
+
+// The bilateral grids of all training views (DESIGN.md section 4.11): grids [views, L, H, W, 12] uploaded at identity,
+// their Adam moments (zero) and the host-side per-view step counts.  A view's grid changes only in the steps that
+// render it.
+class BilateralGrids {
+   public:
+    explicit BilateralGrids(uint32_t num_views, cudaStream_t s = nullptr)
+        : views_(num_views), grids_((size_t)num_views * BG_BILAGRID_FLOATS), m_((size_t)num_views * BG_BILAGRID_FLOATS, true),
+          v_((size_t)num_views * BG_BILAGRID_FLOATS, true), tv_loss_(1, true), steps_(num_views, 0) {
+        if (num_views == 0) throw Error(BG_ERR_INVALID, "BilateralGrids: at least one view");
+        std::vector<float> host((size_t)num_views * BG_BILAGRID_FLOATS, 0.0f);
+        for (size_t c = 0; c < host.size(); c += 12) host[c] = host[c + 5] = host[c + 10] = 1.0f;   // M = I, b = 0
+        grids_.upload(host.data(), host.size(), s);
+        check_cuda(cudaStreamSynchronize(s), "BilateralGrids upload");
+    }
+    uint32_t num_views() const { return views_; }
+    float *grid(uint32_t view) { return grids_.data() + (size_t)check_view(view) * BG_BILAGRID_FLOATS; }
+    float *m(uint32_t view) { return m_.data() + (size_t)check_view(view) * BG_BILAGRID_FLOATS; }
+    float *v(uint32_t view) { return v_.data() + (size_t)check_view(view) * BG_BILAGRID_FLOATS; }
+    int steps(uint32_t view) const { return steps_[check_view(view)]; }
+    const float *tv_loss() const { return tv_loss_.data(); }   // device scalar of the last update
+    // Counts one more step of `view` and returns its BgBilagridStep
+    BgBilagridStep step_args(uint32_t view, float lr, float tv_weight) {
+        BgBilagridStep b;
+        b.grid = grid(view); b.m = m(view); b.v = v(view);
+        b.step = ++steps_[view];
+        b.lr = lr; b.tv_weight = tv_weight;
+        b.tv_loss_out = tv_loss_.data();
+        return b;
+    }
+
+   private:
+    uint32_t check_view(uint32_t view) const {
+        if (view >= views_) throw Error(BG_ERR_INVALID, "BilateralGrids: view index out of range");
+        return view;
+    }
+    uint32_t views_;
+    DeviceBuffer<float> grids_, m_, v_, tv_loss_;
+    std::vector<int> steps_;
 };
 
 // brush-render/src/bounding_box.rs:5-31
@@ -550,6 +600,7 @@ class SplatTrainer {
     // gt_packed: device [h,w] rgba8 (view_to_packed_data, scene.rs:97-136).  Returns the device scalar holding the loss.
     const float *step(Context &ctx, cudaStream_t stream, const Camera &camera, const uint32_t *gt_packed, uint32_t w, uint32_t h,
                       float *transforms, float *sh_coeffs, float *raw_opacities, bool has_alpha = false, bool masked_alpha = false) {
+        refuse_grids("SplatTrainer::step");
         BgTrainStepArgs a = step_args(camera, gt_packed, w, h, transforms, sh_coeffs, raw_opacities, has_alpha, masked_alpha,
                                       bg_train_step_workspace_bytes(n_, k_, w, h));
         check(bg_train_step(ctx.handle(), stream, &a), "SplatTrainer::step");
@@ -567,6 +618,7 @@ class SplatTrainer {
     StepLosses step(Context &ctx, cudaStream_t stream, const Camera &camera, const uint32_t *gt_packed, const float *depth_target,
                     uint32_t depth_valid_count, uint32_t w, uint32_t h, float *transforms, float *sh_coeffs, float *raw_opacities,
                     bool has_alpha = false, bool masked_alpha = false) {
+        refuse_grids("SplatTrainer::step");
         BgTrainStepArgs a = step_args(camera, gt_packed, w, h, transforms, sh_coeffs, raw_opacities, has_alpha, masked_alpha,
                                       bg_train_step_depth_workspace_bytes(n_, k_, w, h));
         BgDepthSupervision d;
@@ -578,8 +630,41 @@ class SplatTrainer {
         last_state_ = a.state_out;
         return {loss_.data(), depth_loss_.data()};
     }
+    // The step with view `view`'s bilateral grid (bg_train_step_bilagrid, DESIGN.md section 4.11): the loss sees the render
+    // sliced by the grid, and the grid is updated after the splats at bilagrid_lr(cfg.bilateral_grid_lr, step,
+    // cfg.total_train_iters).  depth_target may be null (no depth term); otherwise as in the depth overload.  Returns the
+    // device scalars (loss = image loss + depth loss + TV term, depth loss (0 without a target), TV term); the next step
+    // overwrites them.  Requires cfg.bilateral_grid.
+    struct GridStepLosses {
+        const float *loss;
+        const float *depth_loss;
+        const float *tv_loss;
+    };
+    GridStepLosses step(Context &ctx, cudaStream_t stream, const Camera &camera, const uint32_t *gt_packed, BilateralGrids &grids,
+                        uint32_t view, const float *depth_target, uint32_t depth_valid_count, uint32_t w, uint32_t h,
+                        float *transforms, float *sh_coeffs, float *raw_opacities, bool has_alpha = false, bool masked_alpha = false) {
+        if (!cfg_.bilateral_grid) throw Error(BG_ERR_INVALID, "SplatTrainer::step: grids handed in, but cfg.bilateral_grid is off");
+        if (view >= grids.num_views()) throw Error(BG_ERR_INVALID, "SplatTrainer::step: view index out of range");
+        BgTrainStepArgs a = step_args(camera, gt_packed, w, h, transforms, sh_coeffs, raw_opacities, has_alpha, masked_alpha,
+                                      bg_train_step_bilagrid_workspace_bytes(n_, k_, w, h));
+        const BgBilagridStep b = grids.step_args(view, (float)bilagrid_lr(cfg_.bilateral_grid_lr, step_, cfg_.total_train_iters),
+                                                 cfg_.bilateral_grid_tv_weight);
+        BgDepthSupervision d;
+        d.target = depth_target;
+        d.weight = cfg_.depth_loss_weight;
+        d.valid_count = depth_target ? depth_valid_count : 0u;
+        d.depth_loss_out = depth_loss_.data();
+        check(bg_train_step_bilagrid(ctx.handle(), stream, &a, depth_target ? &d : nullptr, &b), "SplatTrainer::step (bilateral grid)");
+        if (!depth_target) check_cuda(cudaMemsetAsync(depth_loss_.data(), 0, sizeof(float), stream), "SplatTrainer::step");
+        last_state_ = a.state_out;
+        return {loss_.data(), depth_loss_.data(), grids.tv_loss()};
+    }
 
    private:
+    // the steps without a grid refuse a configuration that asks for one
+    void refuse_grids(const char *who) const {
+        if (cfg_.bilateral_grid) throw Error(BG_ERR_INVALID, std::string(who) + ": cfg.bilateral_grid needs the step that takes the grids");
+    }
     BgTrainStepArgs step_args(const Camera &camera, const uint32_t *gt_packed, uint32_t w, uint32_t h, float *transforms,
                               float *sh_coeffs, float *raw_opacities, bool has_alpha, bool masked_alpha, uint64_t need) {
         step_ += 1;
@@ -634,9 +719,10 @@ class SplatTrainer {
     // parameters.  gt_packed[i]: device [h,w] rgba8 of view i.  min_scale: optional device [n] Mip-Splatting scale floor.
     const float *step_views(Context &ctx, DpComm *comm, cudaStream_t stream, const std::vector<Camera> &cameras,
                             const std::vector<const uint32_t *> &gt_packed, uint32_t w, uint32_t h, Splats &splats,
-                            const float *min_scale = nullptr, bool has_alpha = false, bool masked_alpha = false) {
+                            const float *min_scale = nullptr, bool has_alpha = false, bool masked_alpha = false,
+                            const BilateralGrids *grids = nullptr) {
         std::vector<BgCamera> cams;
-        BgTrainViewsArgs a = views_args(comm, cameras, gt_packed, w, h, splats, min_scale, has_alpha, masked_alpha, cams, false);
+        BgTrainViewsArgs a = views_args(comm, cameras, gt_packed, w, h, splats, min_scale, has_alpha, masked_alpha, cams, false, grids);
         check(bg_train_step_views(ctx.handle(), comm ? comm->handle() : nullptr, stream, &a), "SplatTrainer::step_views");
         last_state_ = a.state_out;
         return loss_.data();
@@ -653,11 +739,12 @@ class SplatTrainer {
     ViewsLosses step_views(Context &ctx, DpComm *comm, cudaStream_t stream, const std::vector<Camera> &cameras,
                            const std::vector<const uint32_t *> &gt_packed, const std::vector<const float *> &depth_targets,
                            const std::vector<uint32_t> &depth_valid_counts, uint32_t w, uint32_t h, Splats &splats,
-                           const float *min_scale = nullptr, bool has_alpha = false, bool masked_alpha = false) {
+                           const float *min_scale = nullptr, bool has_alpha = false, bool masked_alpha = false,
+                           const BilateralGrids *grids = nullptr) {
         if (depth_targets.size() != cameras.size() || depth_valid_counts.size() != cameras.size())
             throw Error(BG_ERR_INVALID, "SplatTrainer::step_views: one depth target and valid count per camera");
         std::vector<BgCamera> cams;
-        BgTrainViewsArgs a = views_args(comm, cameras, gt_packed, w, h, splats, min_scale, has_alpha, masked_alpha, cams, true);
+        BgTrainViewsArgs a = views_args(comm, cameras, gt_packed, w, h, splats, min_scale, has_alpha, masked_alpha, cams, true, grids);
         std::vector<BgDepthSupervision> d(cameras.size());
         for (size_t i = 0; i < d.size(); i++) {
             d[i].target = depth_targets[i];
@@ -673,7 +760,10 @@ class SplatTrainer {
    private:
     BgTrainViewsArgs views_args(DpComm *comm, const std::vector<Camera> &cameras, const std::vector<const uint32_t *> &gt_packed,
                                 uint32_t w, uint32_t h, Splats &splats, const float *min_scale, bool has_alpha, bool masked_alpha,
-                                std::vector<BgCamera> &cams, bool depth) {
+                                std::vector<BgCamera> &cams, bool depth, const BilateralGrids *grids) {
+        // the multi-view steps have no grid term (DESIGN.md section 7)
+        if (grids) throw Error(BG_ERR_INVALID, "SplatTrainer::step_views: the multi-view step does not train bilateral grids");
+        refuse_grids("SplatTrainer::step_views");
         const uint32_t local = (uint32_t)cameras.size(), world = comm ? (uint32_t)comm->world() : 1u;
         if (local == 0 || gt_packed.size() != cameras.size() || local * world > 16)
             throw Error(BG_ERR_INVALID, "SplatTrainer::step_views: 1..16 views per step in total, one image per camera");

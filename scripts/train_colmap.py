@@ -123,7 +123,7 @@ def make_dataset(root: str, ctx, views: int, w: int, h: int, hidden_n: int, init
 
 def run(device: int = 0, iters: int = 3000, views: int = 200, width: int = 1920, height: int = 1080, hidden_n: int = 1_000_000,
         init_points: int = 500_000, max_splats: int = 2_000_000, refine_every: int = None, root: str = None, quiet: bool = False,
-        keep: bool = False, depth_loss_weight: float = 0.0, write_depths: bool = False) -> dict:
+        keep: bool = False, depth_loss_weight: float = 0.0, write_depths: bool = False, bilateral_grid: bool = False) -> dict:
     import torch
     import brush_b200.render as R
     import brush_b200.train as T
@@ -150,7 +150,8 @@ def run(device: int = 0, iters: int = 3000, views: int = 200, width: int = 1920,
     if refine_every is None:
         refine_every = 200 if iters >= 2000 else max(50, iters // 6)
     cfg = T.TrainConfig(total_train_iters=iters, max_splats=max_splats, refine_every=refine_every,
-                        growth_stop_iter=max(int(iters * 0.8), 1), seed=1, depth_loss_weight=depth_loss_weight)
+                        growth_stop_iter=max(int(iters * 0.8), 1), seed=1, depth_loss_weight=depth_loss_weight,
+                        bilateral_grid=bilateral_grid)
     counts, step_ms = [], []
     marks = {"t": None, "done": 0}
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -180,6 +181,8 @@ def run(device: int = 0, iters: int = 3000, views: int = 200, width: int = 1920,
            "eval": evals[-1] if evals else None}
     if depth_loss_weight > 0:
         res["depth_loss_weight"] = depth_loss_weight
+    if bilateral_grid:
+        res["bilateral_grid"] = True
     if step_ms:
         res["iters_per_s_steps_only"] = sum(s for s, _, _ in step_ms) / (sum(ms for _, ms, _ in step_ms) * 1e-3)
     say(json.dumps(res))
@@ -203,8 +206,10 @@ if __name__ == "__main__":
     ap.add_argument("--keep", action="store_true")
     ap.add_argument("--depth-loss-weight", type=float, default=0.0)
     ap.add_argument("--write-depths", action="store_true")
+    ap.add_argument("--bilateral-grid", action="store_true",
+                    help="learn a per-view bilateral grid (DESIGN.md section 4.11); evaluation adds cc_psnr / cc_ssim")
     a = ap.parse_args()
     r = run(iters=a.iters, views=a.views, width=a.width, height=a.height, hidden_n=a.hidden, init_points=a.init_points,
             max_splats=a.max_splats, refine_every=a.refine_every, root=a.root, keep=a.keep, depth_loss_weight=a.depth_loss_weight,
-            write_depths=a.write_depths)
+            write_depths=a.write_depths, bilateral_grid=a.bilateral_grid)
     print(json.dumps(r))
