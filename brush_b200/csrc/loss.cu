@@ -284,8 +284,9 @@ image_loss_bwd_kernel(LossArgs a, Taps taps, const float *__restrict__ dl_dmap, 
 // The four separable passes are written as STREAMING windows on paired FP32: a thread owns a run of L
 // consecutive outputs of one row (or column), keeps them as (L+1)/2 float2 accumulators -- two neighbouring
 // outputs per register pair -- and walks the L+10 inputs once; input i feeds the output pair (2j, 2j+1) with
-// the tap pair (w[i-2j], w[i-2j-1]), one ffma2_rn with the input broadcast.  Tap pairs sit
-// in the kernel's parameter space; every index is a compile-time constant after unrolling (no local memory).
+// the tap pair (w[i-2j], w[i-2j-1]), one ffma2_rn with the input broadcast.  The tap pairs are a __grid_constant__
+// kernel parameter, read in place from parameter space: every index is a compile-time constant after unrolling (no
+// local copy, no per-device upload, nothing for a CUDA-graph capture to trip over).
 // The accumulation order is therefore by input position, not the reference's (pairs d = 1..5, then the
 // centre): the same sum up to f32 rounding.  Work is cut so that each pass fills the 256 threads once:
 //   P1 horizontal, 5 moments : 52 rows x 4 runs of 11      P2 vertical + SSIM partials: 42 cols x 6 runs of 7
@@ -301,34 +302,33 @@ constexpr int F_THREADS = 256;
 
 struct Chain4 { float c[4]; };
 struct TapPairs { float2 p[12]; };   // p[t] = (w[t], w[t-1]) with w[-1] = w[11] = 0
-__constant__ TapPairs c_tap_pairs;    // set once per device by launch_image_loss_fused
 
 // acc[jp][q] += (w[t], w[t-1]) * v[q]  for every output pair jp this input (relative index IREL) reaches
 template <int NQ, int PAIRS, int IREL>
-__device__ __forceinline__ void window_feed(float2 (&acc)[PAIRS][NQ], const float (&v)[NQ]) {
+__device__ __forceinline__ void window_feed(float2 (&acc)[PAIRS][NQ], const float (&v)[NQ], const TapPairs &tp) {
 #pragma unroll
     for (int jp = 0; jp < PAIRS; jp++) {
         const int t = IREL - 2 * jp;
         if (t >= 0 && t <= 11) {
 #pragma unroll
-            for (int q = 0; q < NQ; q++) acc[jp][q] = ffma2_rn(c_tap_pairs.p[t], make_float2(v[q], v[q]), acc[jp][q]);
+            for (int q = 0; q < NQ; q++) acc[jp][q] = ffma2_rn(tp.p[t], make_float2(v[q], v[q]), acc[jp][q]);
         }
     }
 }
 
 // walks inputs 0 .. 2*PAIRS+9 of a run; load(i, v) fetches the NQ values of input i (zero beyond the staged region)
 template <int NQ, int PAIRS, int IREL = 0, typename Load>
-__device__ __forceinline__ void window_run(float2 (&acc)[PAIRS][NQ], Load load) {
+__device__ __forceinline__ void window_run(float2 (&acc)[PAIRS][NQ], const TapPairs &tp, Load load) {
     if constexpr (IREL < 2 * PAIRS + 10) {
         float v[NQ];
         load(IREL, v);
-        window_feed<NQ, PAIRS, IREL>(acc, v);
-        window_run<NQ, PAIRS, IREL + 1>(acc, load);
+        window_feed<NQ, PAIRS, IREL>(acc, v, tp);
+        window_run<NQ, PAIRS, IREL + 1>(acc, tp, load);
     }
 }
 
 __global__ void __launch_bounds__(F_THREADS, 3)
-image_loss_fused_kernel(LossArgs a, Chain4 chain, float *__restrict__ dl_dpred,
+image_loss_fused_kernel(LossArgs a, Chain4 chain, const __grid_constant__ TapPairs taps, float *__restrict__ dl_dpred,
                         float *__restrict__ loss_partials) {
     extern __shared__ float f_smem[];
     float *buf_a = f_smem, *buf_b = f_smem + F_BUF_A;
@@ -407,7 +407,7 @@ image_loss_fused_kernel(LossArgs a, Chain4 chain, float *__restrict__ dl_dpred,
                 for (int jp = 0; jp < 6; jp++)
 #pragma unroll
                     for (int q = 0; q < 2; q++) acc[jp][q] = make_float2(0.0f, 0.0f);
-                window_run<2, 6>(acc, [&](int i, float (&v)[2]) {
+                window_run<2, 6>(acc, taps, [&](int i, float (&v)[2]) {
                     float x = 0.0f;
                     if (o0 + i < FE) x = src[i * 2];
                     v[0] = x; v[1] = x * x;
@@ -425,7 +425,7 @@ image_loss_fused_kernel(LossArgs a, Chain4 chain, float *__restrict__ dl_dpred,
                 for (int jp = 0; jp < 6; jp++)
 #pragma unroll
                     for (int q = 0; q < 2; q++) acc[jp][q] = make_float2(0.0f, 0.0f);
-                window_run<2, 6>(acc, [&](int i, float (&v)[2]) {
+                window_run<2, 6>(acc, taps, [&](int i, float (&v)[2]) {
                     float y = 0.0f;
                     if (o0 + i < FE) y = src[i * 2 + 1];
                     v[0] = y; v[1] = y * y;
@@ -441,7 +441,7 @@ image_loss_fused_kernel(LossArgs a, Chain4 chain, float *__restrict__ dl_dpred,
                 float2 acc[6][1];
 #pragma unroll
                 for (int jp = 0; jp < 6; jp++) acc[jp][0] = make_float2(0.0f, 0.0f);
-                window_run<1, 6>(acc, [&](int i, float (&v)[1]) {
+                window_run<1, 6>(acc, taps, [&](int i, float (&v)[1]) {
                     float2 xy = make_float2(0.0f, 0.0f);
                     if (o0 + i < FE) xy = *reinterpret_cast<const float2 *>(src + i * 2);
                     v[0] = xy.x * xy.y;
@@ -464,7 +464,7 @@ image_loss_fused_kernel(LossArgs a, Chain4 chain, float *__restrict__ dl_dpred,
 #pragma unroll
                 for (int q = 0; q < 5; q++) acc[jp][q] = make_float2(0.0f, 0.0f);
             const float *src = buf_b + (r0 * FP + px_) * 5;
-            window_run<5, 4>(acc, [&](int i, float (&v)[5]) {
+            window_run<5, 4>(acc, taps, [&](int i, float (&v)[5]) {
                 if (r0 + i < FE) {
 #pragma unroll
                     for (int q = 0; q < 5; q++) v[q] = src[i * FP * 5 + q];
@@ -518,7 +518,7 @@ image_loss_fused_kernel(LossArgs a, Chain4 chain, float *__restrict__ dl_dpred,
 #pragma unroll
                 for (int q = 0; q < 3; q++) acc[jp][q] = make_float2(0.0f, 0.0f);
             const float *src = buf_a + (row * FP + o0) * 3;
-            window_run<3, 3>(acc, [&](int i, float (&v)[3]) {
+            window_run<3, 3>(acc, taps, [&](int i, float (&v)[3]) {
                 if (o0 + i < FP) { v[0] = src[i * 3]; v[1] = src[i * 3 + 1]; v[2] = src[i * 3 + 2]; }
                 else { v[0] = v[1] = v[2] = 0.0f; }
             });
@@ -542,7 +542,7 @@ image_loss_fused_kernel(LossArgs a, Chain4 chain, float *__restrict__ dl_dpred,
 #pragma unroll
                 for (int q = 0; q < 3; q++) acc[jp][q] = make_float2(0.0f, 0.0f);
             const float *src = buf_b + (y0 * FT + x) * 3;
-            window_run<3, 2>(acc, [&](int i, float (&v)[3]) {
+            window_run<3, 2>(acc, taps, [&](int i, float (&v)[3]) {
                 v[0] = src[i * FT * 3]; v[1] = src[i * FT * 3 + 1]; v[2] = src[i * FT * 3 + 2];   // rows y0 .. y0+13 < FP
             });
 #pragma unroll
@@ -627,18 +627,11 @@ cudaError_t launch_image_loss_fused(cudaStream_t s, const float *pred, const uin
     if (e != cudaSuccess) return e;
     Chain4 ch;
     for (uint32_t i = 0; i < 4; i++) ch.c[i] = i < c ? chain_per_channel[i] : 0.0f;
-    static bool taps_set[64] = {};
-    int dev = 0;
-    if ((e = cudaGetDevice(&dev)) != cudaSuccess) return e;
-    if (dev < 64 && !taps_set[dev]) {   // the window weights never change: one upload per device
-        const Taps taps = make_taps();
-        TapPairs tp;
-        for (int t = 0; t < 12; t++) tp.p[t] = make_float2(t <= 10 ? taps.w[t] : 0.0f, t >= 1 ? taps.w[t - 1] : 0.0f);
-        if ((e = cudaMemcpyToSymbol(c_tap_pairs, &tp, sizeof(tp))) != cudaSuccess) return e;
-        taps_set[dev] = true;
-    }
-    image_loss_fused_kernel<<<grid, block, smem, s>>>(make_args(pred, gt, h, w, sc, sy, sx, l1_w, ssim_w, bg, mask), ch, dl_dpred,
-                                                      loss_partials);
+    const Taps taps = make_taps();
+    TapPairs tp;
+    for (int t = 0; t < 12; t++) tp.p[t] = make_float2(t <= 10 ? taps.w[t] : 0.0f, t >= 1 ? taps.w[t - 1] : 0.0f);
+    image_loss_fused_kernel<<<grid, block, smem, s>>>(make_args(pred, gt, h, w, sc, sy, sx, l1_w, ssim_w, bg, mask), ch, tp,
+                                                      dl_dpred, loss_partials);
     return cudaGetLastError();
 }
 

@@ -35,6 +35,13 @@ def _strides_hwc(pred: torch.Tensor):
     return sc, sy, sx
 
 
+def _out_like(pred: torch.Tensor, zero: bool = True) -> torch.Tensor:
+    """An output with pred's shape AND strides: the kernels write dL/dpred through pred's strides, so a padded row pitch
+    (a column slice of a wider image) needs an output with the same pitch, which zeros_like does not give."""
+    out = torch.empty_strided(pred.shape, pred.stride(), dtype=pred.dtype, device=pred.device)
+    return out.zero_() if zero else out
+
+
 def _bg_ptr(cfg: ImageLossConfig):
     if cfg.composite_bg is None:
         return None
@@ -62,7 +69,7 @@ def image_loss_backward(ctx: RenderContext, pred_hwc: torch.Tensor, gt_packed: t
     h, w = pred_hwc.shape[0], pred_hwc.shape[1]
     sc, sy, sx = _strides_hwc(pred_hwc)
     if out_hwc is None:
-        out_hwc = torch.zeros_like(pred_hwc)
+        out_hwc = _out_like(pred_hwc)
     if out_hwc.stride() != pred_hwc.stride():
         raise ValueError("out_hwc must have the strides of pred_hwc")
     dl_dmap = dl_dmap.contiguous()
@@ -85,7 +92,9 @@ def image_loss_fused(ctx: RenderContext, pred_hwc: torch.Tensor, gt_packed: torc
         raise ValueError("gt_packed height/width must match pred")
     sc, sy, sx = _strides_hwc(pred_hwc)
     if out_hwc is None:
-        out_hwc = torch.zeros_like(pred_hwc) if pred_hwc.shape[2] > channels else torch.empty_like(pred_hwc)
+        out_hwc = _out_like(pred_hwc, zero=pred_hwc.shape[2] > channels)
+    if out_hwc.stride() != pred_hwc.stride() or tuple(out_hwc.shape) != tuple(pred_hwc.shape):
+        raise ValueError("out_hwc must have the shape and strides of pred_hwc")
     n_part = int(lib.bg_image_loss_num_partials(channels, h, w))
     partials = torch.empty((channels, n_part // channels), dtype=torch.float32, device=pred_hwc.device)
     chain = (C.c_float * channels)(*[float(x) for x in chain_per_channel])
