@@ -16,7 +16,7 @@ BG_OK, BG_ERR_NULL, BG_ERR_INVALID, BG_ERR_CUDA, BG_ERR_CAPACITY, BG_ERR_UNSUPPO
 PASS_FORWARD, PASS_BACKWARD, PASS_BACKWARD_SMOOTH = 0, 1, 2
 PROJECTED_STRIDE = 16
 VCOMBINED_STRIDE = 10
-ABI_VERSION = 12
+ABI_VERSION = 13
 BILAGRID_L, BILAGRID_H, BILAGRID_W = 8, 16, 16
 BILAGRID_FLOATS = BILAGRID_L * BILAGRID_H * BILAGRID_W * 12
 
@@ -224,6 +224,17 @@ class BgBilagridStep(C.Structure):
     ]
 
 
+class BgBilagridViews(C.Structure):
+    _fields_ = [
+        ("grids", C.c_void_p), ("m", C.c_void_p), ("v", C.c_void_p),
+        ("steps", C.c_void_p),
+        ("num_views", C.c_uint32),
+        ("view_index", C.POINTER(C.c_uint32)),
+        ("lr", C.c_float), ("tv_weight", C.c_float),
+        ("tv_loss_out", C.c_void_p),
+    ]
+
+
 # name -> (restype, argtypes); one entry per function declared in include/brush_b200.h
 _P, _U32, _U64, _I32, _I64, _F = C.c_void_p, C.c_uint32, C.c_uint64, C.c_int32, C.c_int64, C.c_float
 SIGNATURES = {
@@ -301,6 +312,10 @@ SIGNATURES = {
     "bg_bilagrid_update": (_I32, [_P, _P, C.POINTER(BgBilagridStep), _P]),
     "bg_train_step_bilagrid_workspace_bytes": (_U64, [_U32, _U32, _U32, _U32]),
     "bg_train_step_bilagrid": (_I32, [_P, _P, C.POINTER(BgTrainStepArgs), C.POINTER(BgDepthSupervision), C.POINTER(BgBilagridStep)]),
+    "bg_train_step_views_bilagrid_workspace_bytes": (_U64, [_U32, _U32, _U32, _U32, _U32, _U32]),
+    "bg_train_step_views_bilagrid": (_I32, [_P, _P, _P, C.POINTER(BgTrainViewsArgs), C.POINTER(BgDepthSupervision),
+                                            C.POINTER(BgBilagridViews)]),
+    "bg_bilagrid_update_views": (_I32, [_P, _P, C.POINTER(BgBilagridViews), _U32, _P, _P]),
 }
 
 _lib = None

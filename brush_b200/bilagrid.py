@@ -5,6 +5,7 @@ the loss, learned with the splats and not part of the model: evaluation and expo
   BilateralGrids          grids [views, L, H, W, 12] at identity, their Adam moments, each view's own step count
   slice / slice_backward  bg_bilagrid_slice / bg_bilagrid_slice_backward
   update                  bg_bilagrid_update: TV gradient and value, then Adam on one view's grid
+  update_views            bg_bilagrid_update_views: the same for several gradient slots in one launch, a view's slots summed
   apply_bilateral_grid    a training view's render as the model explains it (the raw render sliced by its grid)
   bilagrid_lr             the learning-rate schedule: warm-up over 1000 steps, then exponential decay
 """
@@ -34,8 +35,13 @@ def identity_grids(num_views: int, device) -> torch.Tensor:
 
 
 class BilateralGrids:
-    """The grids of all training views, their Adam moments and the host-side per-view step counts.  A view's grid
-    changes only in the steps that render that view."""
+    """The grids of all training views, their Adam moments and the per-view step counts.  A view's grid changes only in
+    the steps that render that view, and its count is the number of those steps.
+
+    The counts are kept twice: `steps`, a host list that the single-view steps advance, and `device_steps`, int32
+    [views] that the multi-view steps advance on the device (a rank does not know the other ranks' views).  Each copy is
+    brought up to date from the other only when a step of the other kind ran since: a 4 * views byte transfer when the
+    path changes, none in a steady run of either."""
 
     def __init__(self, num_views: int, device):
         if num_views < 1:
@@ -44,9 +50,35 @@ class BilateralGrids:
         self.grids = identity_grids(self.num_views, device)
         self.m = torch.zeros_like(self.grids)
         self.v = torch.zeros_like(self.grids)
-        self.steps = [0] * self.num_views
+        self._steps = [0] * self.num_views
+        self._device_steps = torch.zeros(self.num_views, dtype=torch.int32, device=self.grids.device)
+        self._current = "both"   # which copy of the counts is up to date: "host", "device" or "both"
         self.v_grid = torch.zeros((L, H, W, 12), dtype=torch.float32, device=self.grids.device)
         self.tv_loss = torch.zeros(1, dtype=torch.float32, device=self.grids.device)
+        self.views_tv_loss = torch.zeros(16, dtype=torch.float32, device=self.grids.device)
+
+    @property
+    def steps(self) -> list:
+        """Each view's step count, as a host list (read back once after multi-view steps)."""
+        if self._current == "device":
+            self._steps = [int(x) for x in self._device_steps.tolist()]
+            self._current = "both"
+        return self._steps
+
+    @property
+    def device_steps(self) -> torch.Tensor:
+        """Each view's step count, int32 [views] on the device (written once after single-view steps).  Whoever reads it
+        for a step that advances it on the device calls advance_on_device() first."""
+        if self._current == "host":
+            self._device_steps.copy_(torch.tensor(self._steps, dtype=torch.int32))
+            self._current = "both"
+        return self._device_steps
+
+    def advance_on_device(self) -> torch.Tensor:
+        """device_steps, marked as the only up-to-date copy: the caller's step advances it on the device."""
+        t = self.device_steps
+        self._current = "device"
+        return t
 
     def check_view(self, view: int) -> int:
         if not 0 <= view < self.num_views:
@@ -56,12 +88,29 @@ class BilateralGrids:
     def step_args(self, view: int, lr: float, tv_weight: float) -> "_lib.BgBilagridStep":
         """Counts one more step of `view` and returns its BgBilagridStep (tv_loss_out -> self.tv_loss)."""
         view = self.check_view(view)
-        self.steps[view] += 1
+        steps = self.steps
+        steps[view] += 1
+        self._current = "host"
         a = _lib.BgBilagridStep()
         a.grid, a.m, a.v = (t[view].data_ptr() for t in (self.grids, self.m, self.v))
-        a.step, a.lr, a.tv_weight = self.steps[view], float(lr), float(tv_weight)
+        a.step, a.lr, a.tv_weight = steps[view], float(lr), float(tv_weight)
         a.tv_loss_out = self.tv_loss.data_ptr()
         return a
+
+    def views_args(self, view_index, lr: float, tv_weight: float, tv_out: torch.Tensor):
+        """The BgBilagridViews of a step (or an update) whose counts advance on the device; view_index: the local views'
+        training-view indices (None for bg_bilagrid_update_views).  Returns it with the host array it points into."""
+        a = _lib.BgBilagridViews()
+        a.grids, a.m, a.v = self.grids.data_ptr(), self.m.data_ptr(), self.v.data_ptr()
+        a.steps = self.advance_on_device().data_ptr()
+        a.num_views = self.num_views
+        idx = None
+        if view_index is not None:
+            idx = (C.c_uint32 * len(view_index))(*[self.check_view(v) for v in view_index])
+            a.view_index = idx
+        a.lr, a.tv_weight = float(lr), float(tv_weight)
+        a.tv_loss_out = tv_out.data_ptr()
+        return a, idx
 
 
 def _check(t: torch.Tensor, name: str, shape, device) -> torch.Tensor:
@@ -128,6 +177,25 @@ def update(ctx: RenderContext, grids: BilateralGrids, view: int, v_grid: torch.T
     _lib.check(_lib.load().bg_bilagrid_update(ctx.handle, _stream_ptr(ctx.device), C.byref(a), v_grid.data_ptr()),
                "bg_bilagrid_update")
     return grids.tv_loss[0]
+
+
+def update_views(ctx: RenderContext, grids: BilateralGrids, slot_view, v_grids: torch.Tensor, lr: float,
+                 tv_weight: float) -> torch.Tensor:
+    """One update of every view named in slot_view (1..16 training-view indices, one per gradient slot of v_grids
+    [slots, L, H, W, 12]): a view's slots summed in slot order (into its first slot), TV, then Adam with the view's count
+    + 1, bit-identical to update() given that sum; each named view's count advances by one.  Returns the device [slots]
+    TV values (every slot of a view gets its view's value)."""
+    slot_view = [grids.check_view(v) for v in slot_view]
+    if not 1 <= len(slot_view) <= 16:
+        raise ValueError("update_views takes 1..16 slots")
+    dev = grids.grids.device
+    _check(v_grids, "v_grids", (len(slot_view), L, H, W, 12), dev)
+    sv = torch.tensor(slot_view, dtype=torch.int32, device=dev)
+    tv = torch.empty(len(slot_view), dtype=torch.float32, device=dev)
+    a, _ = grids.views_args(None, lr, tv_weight, tv)
+    _lib.check(_lib.load().bg_bilagrid_update_views(ctx.handle, _stream_ptr(ctx.device), C.byref(a), len(slot_view), sv.data_ptr(),
+                                                    v_grids.data_ptr()), "bg_bilagrid_update_views")
+    return tv
 
 
 def apply_bilateral_grid(ctx: RenderContext, out_img: torch.Tensor, grids: BilateralGrids, view: int) -> torch.Tensor:

@@ -10,6 +10,7 @@
 #include <cstring>
 #include <new>
 
+#include "bg_adam.cuh"
 #include "bg_common.cuh"
 #include "bg_project.cuh"
 #include "bg_dp.cuh"
@@ -557,19 +558,6 @@ extern "C" int32_t bg_depth_loss_fused(BgContext *c, void *stream, const float *
     return BG_OK;
 }
 
-// compiler-rt __powisf2, what Rust's f32::powi lowers to (adam_scaled.rs:135-142)
-static float powi_f32(float a, int b) {
-    const bool recip = b < 0;
-    float r = 1.0f;
-    while (true) {
-        if (b & 1) r *= a;
-        b /= 2;
-        if (b == 0) break;
-        a *= a;
-    }
-    return recip ? 1.0f / r : r;
-}
-
 extern "C" int32_t bg_adam_step(BgContext *c, void *stream, float *p, const float *g, float *m, float *v,
                                 uint64_t rows, uint32_t cols, const float *lr_scale, float lr, float beta1, float beta2,
                                 float eps, int32_t t, int32_t reduce_v) {
@@ -645,7 +633,7 @@ extern "C" int32_t bg_normal_noise(BgContext *c, void *stream, uint64_t seed, ui
 
 // The update pass over all n Gaussians of `a` (BgTrainUpdateArgs, BgTrainStepArgs or BgTrainViewsArgs, which name the
 // trainable state and the schedule alike): the state pointers and the step-dependent constants, unit gradient scales.
-// The caller sets the gradient sources.  compiler-rt __powisf2 is defined above (powi_f32).
+// The caller sets the gradient sources.  compiler-rt __powisf2 is powi_f32 (bg_adam.cuh).
 template <class A>
 static UpdateParams update_params(const A *a) {
     UpdateParams P;
@@ -1094,13 +1082,44 @@ ViewsWs carve_views_ws(void *base, uint32_t n, uint32_t w, uint32_t h, uint32_t 
     ws.bytes = cv.off;
     return ws;
 }
+
+// The bilateral grids' scratch of bg_train_step_views_bilagrid, behind the views-depth workspace: the sliced image, the
+// send slots (one per local view: its grid gradient, then its view index as raw bits, padded to keep the slots 16-byte
+// aligned) and, with world > 1, the gathered slots of all views in global order.
+constexpr uint32_t GRID_SLOT = BG_BILAGRID_FLOATS + 4;
+struct ViewsGridWs {
+    float *sliced, *send, *recv;
+    uint64_t bytes;
+};
+ViewsGridWs carve_views_grid_ws(void *base, uint64_t off, uint32_t w, uint32_t h, uint32_t local, uint32_t world) {
+    Carver cv{base, off};
+    ViewsGridWs ws;
+    ws.sliced = cv.take((uint64_t)w * h * 4);
+    ws.send = cv.take((uint64_t)local * GRID_SLOT);
+    ws.recv = cv.take(world > 1 ? (uint64_t)local * world * GRID_SLOT : 0);
+    ws.bytes = cv.off;
+    return ws;
+}
+
+// the checks of BgBilagridViews shared by the step and the operator; local_views > 0 checks the step's view indices
+int32_t check_bilagrid_views(const BgBilagridViews *g, uint32_t local_views, const char *who) {
+    if (!g || !g->grids || !g->m || !g->v || !g->steps || !g->tv_loss_out || (local_views && !g->view_index)) return BG_ERR_NULL;
+    if (g->num_views == 0) return invalid(who, "num_views must be >= 1");
+    if (!(g->lr >= 0.0f) || !std::isfinite(g->lr) || !(g->tv_weight >= 0.0f) || !std::isfinite(g->tv_weight))
+        return invalid(who, "bilateral grid lr and tv_weight must be finite and >= 0");
+    if (!aligned16(g->grids) || !aligned16(g->m) || !aligned16(g->v) || (uintptr_t)g->steps % 4)
+        return invalid(who, "grids, m and v must be 16-byte aligned, steps 4-byte aligned");
+    for (uint32_t i = 0; i < local_views; i++)
+        if (g->view_index[i] >= g->num_views) return invalid(who, "view_index out of range (>= num_views)");
+    return BG_OK;
+}
 }  // namespace
 
 // BG_DP_TRACE=1: device timeline of the multi-device step (stderr, rank 0 only; synchronises -- a debugging aid)
 namespace {
 struct DpTrace {
     bool on = false;
-    cudaEvent_t e[12] = {};
+    cudaEvent_t e[13] = {};
     DpTrace() {
         const char *v = getenv("BG_DP_TRACE");
         on = v && v[0] == '1';
@@ -1114,10 +1133,11 @@ struct DpTrace {
         if (!on) return;
         cudaStreamSynchronize(s); cudaStreamSynchronize(cs);
         if (rank != 0) return;
-        static const char *names[12] = {"step start", "blend bwd + colour pack done", "project bwd + row pack done", "records arrived (s)",
+        static const char *names[13] = {"step start", "blend bwd + colour pack done", "project bwd + row pack done", "records arrived (s)",
                                         "update part 1 done", "sums arrived (s)", "update part 2 done", "all-gather start (comm)",
-                                        "all-gather end (comm)", "all-reduce start (comm)", "all-reduce end (comm)", ""};
-        for (int i = 1; i < 11; i++) {
+                                        "all-gather end (comm)", "all-reduce start (comm)", "all-reduce end (comm)",
+                                        "grid gather start (comm)", "grid gather end (comm)"};
+        for (int i = 1; i < 13; i++) {
             float ms = 0.0f;
             if (e[i] && cudaEventElapsedTime(&ms, e[0], e[i]) == cudaSuccess) fprintf(stderr, "[bg dp trace] %-32s %8.3f ms\n", names[i], ms);
         }
@@ -1137,10 +1157,18 @@ extern "C" uint64_t bg_train_step_views_depth_workspace_bytes(uint32_t n, uint32
     return carve_depth_ws(nullptr, bg_train_step_views_workspace_bytes(n, k, w, h, local, world), n, w, h).bytes;
 }
 
+extern "C" uint64_t bg_train_step_views_bilagrid_workspace_bytes(uint32_t n, uint32_t k, uint32_t w, uint32_t h, uint32_t local,
+                                                                 uint32_t world) {
+    return carve_views_grid_ws(nullptr, bg_train_step_views_depth_workspace_bytes(n, k, w, h, local, world), w, h, std::max(local, 1u),
+                               std::max(world, 1u)).bytes;
+}
+
 // The multi-view step.  dep == nullptr: bg_train_step_views.  Otherwise dep[local_views] (validated by
 // bg_train_step_views_depth); a view whose term runs renders depth and folds its depth gradient into the exchange row, the
-// other views run exactly the plain view's launches.
-static int32_t train_step_views(BgContext *c, BgDpComm *h, void *stream, BgTrainViewsArgs *a, const BgDepthSupervision *dep) {
+// other views run exactly the plain view's launches.  gr: the views' bilateral grids (validated by
+// bg_train_step_views_bilagrid) or null.
+static int32_t train_step_views(BgContext *c, BgDpComm *h, void *stream, BgTrainViewsArgs *a, const BgDepthSupervision *dep,
+                                const BgBilagridViews *gr) {
     if (!c || !a || !a->cams) return BG_ERR_NULL;
     if (int32_t r = check_train_args(a, "bg_train_step_views"); r != BG_OK) return r;
     const uint32_t n = a->n, k = a->k, w = a->w, hh = a->h, local = a->local_views;
@@ -1159,6 +1187,11 @@ static int32_t train_step_views(BgContext *c, BgDpComm *h, void *stream, BgTrain
     const DepthWs dws = carve_depth_ws(a->workspace, bg_train_step_views_workspace_bytes(n, k, w, hh, local, world), n, w, hh);
     if (int32_t r = check_workspace_bytes("bg_train_step_views_depth", "bg_train_step_views_depth_workspace_bytes", a->workspace_bytes,
                                           dep ? dws.bytes : 0); r != BG_OK)
+        return r;
+    const ViewsGridWs gws = carve_views_grid_ws(gr ? a->workspace : nullptr, bg_train_step_views_depth_workspace_bytes(n, k, w, hh, local, world),
+                                                w, hh, local, world);
+    if (int32_t r = check_workspace_bytes("bg_train_step_views_bilagrid", "bg_train_step_views_bilagrid_workspace_bytes",
+                                          a->workspace_bytes, gr ? gws.bytes : 0); r != BG_OK)
         return r;
     cudaStream_t s = (cudaStream_t)stream;
     BG_CUDA(cudaSetDevice(c->device));
@@ -1179,6 +1212,12 @@ static int32_t train_step_views(BgContext *c, BgDpComm *h, void *stream, BgTrain
     for (uint32_t i = 0; i < local; i++)
         for (int q = 0; q < 3; q++) hdr.pos[i][q] = a->cams[i].cam_pos[q];
     BG_CUDA(launch_write_header(s, ws.hdr, hdr, local));
+    if (gr) {
+        DpGridIndex gi;
+        memset(&gi, 0, sizeof(gi));
+        for (uint32_t i = 0; i < local; i++) gi.view[i] = gr->view_index[i];
+        BG_CUDA(launch_write_grid_index(s, gws.send + BG_BILAGRID_FLOATS, GRID_SLOT, gi, local));
+    }
     DpComm *d = world > 1 ? h->c : nullptr;
     DpTrace &tr = g_dp_trace;
     if (d) tr.mark(0, s);
@@ -1186,6 +1225,8 @@ static int32_t train_step_views(BgContext *c, BgDpComm *h, void *stream, BgTrain
     // leave as soon as the last local view's blend backward is done and travel UNDER its projection backward; the summed
     // small rows and the MAX statistics (all-reduces) follow once that is done.  The update pass is split the same way:
     // the SH part (70 % of its traffic) needs the records only and runs under the all-reduces, the rest follows them.
+    // With bilateral grids the slots of the grid gradients are gathered first, as soon as the last local view's slice
+    // backward is done: they travel under its blend and projection backward.
     bool alpha_dirty = false;   // a depth view added to v_output[...,3], which the 3-channel image loss leaves as it is
     for (uint32_t i = 0; i < local; i++) {
         const BgCamera *cam = a->cams + i;
@@ -1196,7 +1237,21 @@ static int32_t train_step_views(BgContext *c, BgDpComm *h, void *stream, BgTrain
         r = render_forward(c, stream, cam, w, hh, n, k, r_t, a->sh, r_o, a->mip, a->background, BG_PASS_BACKWARD, ws.out_img, vd.depth,
                            ws.visible, ws.max_radius, &a->state_out);
         if (r != BG_OK) return r;
-        if ((r = view_loss(c, stream, a, a->gt_packed[i], ws, ws.out_img, ws.loss_terms + i, di, dws)) != BG_OK) return r;
+        const float *grid = gr ? gr->grids + (size_t)gr->view_index[i] * BG_BILAGRID_FLOATS : nullptr;
+        if (gr) BG_CUDA(launch_bilagrid_slice(s, grid, ws.out_img, w, hh, gws.sliced));
+        if ((r = view_loss(c, stream, a, a->gt_packed[i], ws, gr ? gws.sliced : ws.out_img, ws.loss_terms + i, di, dws)) != BG_OK) return r;
+        if (gr) {
+            // back through the slice in place (the blend backward replays the RAW render); the grid gradient into slot i
+            BG_CUDA(launch_bilagrid_slice_bwd(s, grid, ws.out_img, ws.v_output, w, hh, ws.v_output, gws.send + (size_t)i * GRID_SLOT));
+            if (d && i + 1 == local) {
+                BG_CUDA(cudaEventRecord(d->ev_ready, s));
+                BG_CUDA(cudaStreamWaitEvent(d->stream, d->ev_ready, 0));
+                tr.mark(11, d->stream);
+                const int rc = dp_exchange_grids(d, (size_t)local * GRID_SLOT, gws.send, gws.recv);
+                if (rc != 0) return nccl_fail("bg_train_step_views_bilagrid: exchange (grids)", rc);
+                tr.mark(12, d->stream);
+            }
+        }
         r = rasterize_backward(c, stream, &a->state_out, ws.out_img, vd.depth, ws.v_output, vd.v_depth, a->background, 0, ws.v_combined, n,
                                vd.v_z, di ? "bg_rasterize_backward_depth" : "bg_rasterize_backward");
         if (r != BG_OK) return r;
@@ -1220,6 +1275,14 @@ static int32_t train_step_views(BgContext *c, BgDpComm *h, void *stream, BgTrain
         else
             BG_CUDA(launch_pack_view(s, n, local, i, i == 0, ws.v_t, ws.v_o, nullptr, ws.v_refine, ws.visible, ws.max_radius, ws.small,
                                      ws.stat, ws.record));
+    }
+    if (gr) {
+        // every rank updates the grids of all views of the step from the same slots in global order
+        float *slots = d ? gws.recv : gws.send;
+        if (d) BG_CUDA(cudaStreamWaitEvent(s, d->ev_chunk[2], 0));
+        BG_CUDA(launch_bilagrid_update_views(s, gr->grids, gr->m, gr->v, gr->steps, gr->num_views, gr->lr, gr->tv_weight, slots,
+                                             GRID_SLOT, reinterpret_cast<const uint32_t *>(slots + BG_BILAGRID_FLOATS), GRID_SLOT,
+                                             views, d ? (uint32_t)d->rank * local : 0u, local, gr->tv_loss_out, ws.loss_terms));
     }
     BG_CUDA(launch_loss_mean(s, ws.loss_terms, local, a->loss_out));
     UpdateParams P = update_params(a);
@@ -1260,22 +1323,54 @@ static int32_t train_step_views(BgContext *c, BgDpComm *h, void *stream, BgTrain
 }
 
 extern "C" int32_t bg_train_step_views(BgContext *c, BgDpComm *h, void *stream, BgTrainViewsArgs *a) {
-    return train_step_views(c, h, stream, a, nullptr);
+    return train_step_views(c, h, stream, a, nullptr, nullptr);
 }
 
 // ---- bg_train_step_views_depth: bg_train_step_views with the depth term of DESIGN.md section 4.7 on the views that carry one.
 // The depth gradient reaches v_transforms[:, 0:3] and the refine weight only, both already in the exchanged rows: the
 // exchange is unchanged, and ranks with and without depth views share a step.
+static int32_t check_views_depth(const BgTrainViewsArgs *a, const BgDepthSupervision *depth, const char *who) {
+    for (uint32_t i = 0; i < a->local_views; i++) {
+        if (int32_t r = check_depth(depth[i], who); r != BG_OK) return r;
+        if (depth_term(depth[i]) && (uintptr_t)depth[i].target % 4) return invalid(who, "target must be 4-byte aligned");
+    }
+    return BG_OK;
+}
+
 extern "C" int32_t bg_train_step_views_depth(BgContext *c, BgDpComm *h, void *stream, BgTrainViewsArgs *a, const BgDepthSupervision *depth) {
     if (!c || !a || !depth) return BG_ERR_NULL;
     const uint32_t local = a->local_views;
     if (local == 0 || local > DP_MAX_VIEWS) return invalid("bg_train_step_views_depth", "1..16 views per step in total");
-    for (uint32_t i = 0; i < local; i++) {
-        if (int32_t r = check_depth(depth[i], "bg_train_step_views_depth"); r != BG_OK) return r;
-        if (depth_term(depth[i]) && (uintptr_t)depth[i].target % 4)
-            return invalid("bg_train_step_views_depth", "target must be 4-byte aligned");
-    }
-    return train_step_views(c, h, stream, a, depth);
+    if (int32_t r = check_views_depth(a, depth, "bg_train_step_views_depth"); r != BG_OK) return r;
+    return train_step_views(c, h, stream, a, depth, nullptr);
+}
+
+// ---- bg_train_step_views_bilagrid: the multi-view step with the views' bilateral grids (DESIGN.md section 4.11), with or
+// without the depth term
+extern "C" int32_t bg_train_step_views_bilagrid(BgContext *c, BgDpComm *h, void *stream, BgTrainViewsArgs *a,
+                                                const BgDepthSupervision *depth, const BgBilagridViews *grids) {
+    const char *who = "bg_train_step_views_bilagrid";
+    if (!c || !a || !grids) return BG_ERR_NULL;
+    const uint32_t local = a->local_views;
+    if (local == 0 || local > DP_MAX_VIEWS) return invalid(who, "1..16 views per step in total");
+    if (int32_t r = check_bilagrid_views(grids, local, who); r != BG_OK) return r;
+    if (depth)
+        if (int32_t r = check_views_depth(a, depth, who); r != BG_OK) return r;
+    return train_step_views(c, h, stream, a, depth, grids);
+}
+
+extern "C" int32_t bg_bilagrid_update_views(BgContext *c, void *stream, const BgBilagridViews *grids, uint32_t slots,
+                                            const uint32_t *slot_view, float *v_grids) {
+    const char *who = "bg_bilagrid_update_views";
+    if (!c || !slot_view || !v_grids) return BG_ERR_NULL;
+    if (int32_t r = check_bilagrid_views(grids, 0, who); r != BG_OK) return r;
+    if (slots == 0 || slots > DP_MAX_VIEWS) return invalid(who, "1..16 slots");
+    if (!aligned16(v_grids) || (uintptr_t)slot_view % 4) return invalid(who, "v_grids must be 16-byte aligned, slot_view 4-byte aligned");
+    BG_CUDA(cudaSetDevice(c->device));
+    BG_CUDA(launch_bilagrid_update_views((cudaStream_t)stream, grids->grids, grids->m, grids->v, grids->steps, grids->num_views,
+                                         grids->lr, grids->tv_weight, v_grids, BG_BILAGRID_FLOATS, slot_view, 1, slots, 0, slots,
+                                         grids->tv_loss_out, nullptr));
+    return BG_OK;
 }
 
 // ---- refine (refine.cu): every decision on the device, one readback of the counts at the end

@@ -20,6 +20,8 @@ struct DpComm {
 };
 
 struct DpHeader { float pos[DP_MAX_VIEWS][3]; };
+// the global training-view index of each local view (its bilateral grid)
+struct DpGridIndex { uint32_t view[DP_MAX_VIEWS]; };
 
 // Exchange buffers (see dp.cu), interleaved per Gaussian so that a slice of the Gaussian range is ONE contiguous piece
 // of each buffer:
@@ -54,7 +56,12 @@ int dp_exchange_chunk(DpComm *cm, uint32_t n, uint32_t local, uint32_t chunks, u
 int dp_exchange_gather(DpComm *cm, uint32_t n, uint32_t local, const float *record, float *recv);
 int dp_exchange_reduce(DpComm *cm, uint32_t n, float *small, float *stat);
 int dp_exchange_header(DpComm *cm, uint32_t local, const float *hdr, float *hdr_all);
+// The multi-view step's bilateral-grid slots: all-gather of `floats` per rank (each local view's grid gradient and its view
+// index), ev_chunk[2] recorded behind it.
+int dp_exchange_grids(DpComm *cm, size_t floats, const float *send, float *recv);
 cudaError_t launch_write_header(cudaStream_t s, float *hdr, const DpHeader &h, uint32_t local);
+// slots[i * stride] = the bits of idx.view[i], i < local
+cudaError_t launch_write_grid_index(cudaStream_t s, float *slots, uint32_t stride, const DpGridIndex &idx, uint32_t local);
 cudaError_t launch_pack_view(cudaStream_t s, uint32_t n, uint32_t local, uint32_t li, bool first, const float *v_t, const float *v_o,
                              const float *v_color, const float *v_refine, const float *visible, const float *max_radius, float *small,
                              float *stat, float *record);

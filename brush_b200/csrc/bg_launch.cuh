@@ -233,5 +233,14 @@ cudaError_t launch_bilagrid_slice_bwd(cudaStream_t s, const float *grid, const f
                                       uint32_t h, float *v_img, float *v_grid);
 // v_grid += tv_weight * dTV/dgrid; *tv_out = tv_weight * TV(grid); *loss_out (may be null) += the same
 cudaError_t launch_bilagrid_tv(cudaStream_t s, const float *grid, float *v_grid, float tv_weight, float *tv_out, float *loss_out);
+// The grid update of the multi-view step (DESIGN.md section 4.11), one launch for all `slots` gradient slots: slot j is
+// v_slots + j * slot_stride ([L,H,W,12], += the TV gradient) of view slot_view[j * view_stride] (device).  Each distinct view
+// takes ONE update: the sum of its slots in slot order, TV then Adam (bilagrid_tv_kernel's and adam_kernel's rounding, the
+// bias corrections of steps[view] + 1), steps[view] += 1.  tv_out [out_count] (and loss_terms, may be null, +=) gets the TV
+// value of slots out_begin.. out_begin + out_count - 1.  grids / m / v: [num_views][L,H,W,12].
+cudaError_t launch_bilagrid_update_views(cudaStream_t s, float *grids, float *m, float *v, int32_t *steps, uint32_t num_views,
+                                         float lr, float tv_weight, float *v_slots, uint32_t slot_stride, const uint32_t *slot_view,
+                                         uint32_t view_stride, uint32_t slots, uint32_t out_begin, uint32_t out_count,
+                                         float *tv_out, float *loss_terms);
 
 }  // namespace bg

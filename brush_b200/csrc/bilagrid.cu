@@ -6,14 +6,19 @@
 //                              lattice nodes in shared memory (one copy per lane where it fits, so that the
 //                              shared atomics of a warp's lanes never meet on one address) and flushes them with
 //                              one global atomic per node
-//   bilagrid_tv_kernel         one CTA: adds the total-variation gradient to v_grid, writes L_tv (and adds it to a loss)
+//   bilagrid_tv_kernel         one CTA per gradient slot: adds the total-variation gradient to v_grid, writes L_tv (and
+//                              adds it to a loss).  In the grid update of the multi-view step the first slot of each view
+//                              also sums the view's other slots first and runs the Adam step of adam_kernel after, with
+//                              the bias corrections of the view's device-side step count
 #include <cuda_runtime.h>
 
 #include <stdint.h>
 
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 
+#include "bg_adam.cuh"
 #include "bg_launch.cuh"
 
 namespace bg {
@@ -171,10 +176,10 @@ __global__ void __launch_bounds__(BWD_THREADS) bilagrid_slice_bwd_kernel(const f
     }
 }
 
-// TV(G) = sum over axes of (1/P_axis) sum (dG)^2; v_grid += tv_weight * dTV/dG; *tv_out = tv_weight * TV; *loss_out
-// (may be null) += the same.  One CTA, so the value is the same bits every run.
-__global__ void __launch_bounds__(TV_THREADS) bilagrid_tv_kernel(const float *__restrict__ grid, float *__restrict__ v_grid,
-                                                                float tv_weight, float *tv_out, float *loss_out) {
+// TV(G) = sum over axes of (1/P_axis) sum (dG)^2; v_grid += tv_weight * dTV/dG; returns tv_weight * TV in thread 0.  One
+// CTA of TV_THREADS threads in a fixed reduction order, so the value is the same bits every run; thread t handles the
+// elements t + j * TV_THREADS of v_grid.  Ends after a barrier that follows the last read of grid.
+__device__ __forceinline__ float bilagrid_tv(const float *grid, float *v_grid, float tv_weight) {
     constexpr float inv_pz = 1.0f / (float)(GC * (GL - 1) * GH * GW);
     constexpr float inv_py = 1.0f / (float)(GC * GL * (GH - 1) * GW);
     constexpr float inv_px = 1.0f / (float)(GC * GL * GH * (GW - 1));
@@ -211,12 +216,59 @@ __global__ void __launch_bounds__(TV_THREADS) bilagrid_tv_kernel(const float *__
     if (threadIdx.x < 32) {
         part = s_part[threadIdx.x];
         for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-        if (threadIdx.x == 0) {
-            const float tv = tv_weight * part;
-            *tv_out = tv;
-            if (loss_out) *loss_out += tv;
+    }
+    return tv_weight * part;
+}
+
+// CTA j: gradient slot j, a.v_slots + j * slot_stride, of view a.slot_view[j * view_stride] (view 0 when slot_view is
+// null).  The first slot of a view owns it: it adds the gradients of the view's later slots to its own in slot order and
+// the TV gradient of the view's grid; every slot of the view in [out_begin, out_begin + out_count) gets the TV value in
+// tv_out (and added to loss, when not null).  With a.m set the owner then runs one Adam step with the view's count + 1
+// (adam_kernel's arithmetic, the bias corrections formed on the device) and advances the count; without, the caller runs
+// Adam itself (bg_bilagrid_update).  A view >= num_views is skipped.
+struct TvArgs {
+    float *grids, *m, *v;
+    int32_t *steps;
+    uint32_t num_views;
+    float lr, tv_weight;
+    float *v_slots;
+    const uint32_t *slot_view;
+    uint32_t slot_stride, view_stride, slots, out_begin, out_count;
+    float *tv_out, *loss;
+};
+
+__global__ void __launch_bounds__(TV_THREADS) bilagrid_tv_kernel(TvArgs a) {
+    constexpr int N = GL * GH * GW * GC;
+    const uint32_t j = blockIdx.x;
+    auto view_of = [&](uint32_t q) { return a.slot_view ? a.slot_view[(size_t)q * a.view_stride] : 0u; };
+    const uint32_t view = view_of(j);
+    if (view >= a.num_views) return;
+    for (uint32_t q = 0; q < j; q++)
+        if (view_of(q) == view) return;
+    float *g = a.v_slots + (size_t)j * a.slot_stride;
+    for (uint32_t q = j + 1; q < a.slots; q++) {
+        if (view_of(q) != view) continue;
+        const float *o = a.v_slots + (size_t)q * a.slot_stride;
+        for (int i = threadIdx.x; i < N; i += TV_THREADS) g[i] += o[i];
+    }
+    const int32_t t = a.m ? a.steps[view] + 1 : 0;
+    float *grid = a.grids + (size_t)view * N;
+    const float tv = bilagrid_tv(grid, g, a.tv_weight);
+    if (threadIdx.x == 0) {
+        if (a.m) a.steps[view] = t;
+        for (uint32_t q = j; q < a.slots; q++) {
+            if (view_of(q) != view || q < a.out_begin || q - a.out_begin >= a.out_count) continue;
+            a.tv_out[q - a.out_begin] = tv;
+            if (a.loss) a.loss[q - a.out_begin] += tv;
         }
     }
+    if (!a.m) return;
+    // Adam as adam_kernel runs it for bg_bilagrid_update (betas 0.9, 0.999, eps 1e-15, no per-column scale)
+    AdamConsts k;
+    k.lr = a.lr; k.beta1 = 0.9f; k.beta2 = 0.999f; k.eps = 1e-15f; k.f1 = 1.0f - k.beta1; k.f2 = 1.0f - k.beta2;
+    k.bc1 = adam_bias_correction(k.beta1, t); k.bc2 = adam_bias_correction(k.beta2, t); k.first = t == 1;
+    float *mv = a.m + (size_t)view * N, *vv = a.v + (size_t)view * N;
+    for (int i = threadIdx.x; i < N; i += TV_THREADS) adam_element(grid[i], g[i], mv[i], vv[i], k, k.lr);
 }
 
 // The CTA tile of the slice backward for an image w x h: BWD_TX x BWD_TY pixels, a shared box of nx x ny x L lattice
@@ -268,7 +320,26 @@ cudaError_t launch_bilagrid_slice_bwd(cudaStream_t s, const float *grid, const f
 }
 
 cudaError_t launch_bilagrid_tv(cudaStream_t s, const float *grid, float *v_grid, float tv_weight, float *tv_out, float *loss_out) {
-    bilagrid_tv_kernel<<<1, TV_THREADS, 0, s>>>(grid, v_grid, tv_weight, tv_out, loss_out);
+    TvArgs a;
+    memset(&a, 0, sizeof(a));
+    a.grids = const_cast<float *>(grid);   // read only without a.m
+    a.num_views = 1; a.tv_weight = tv_weight;
+    a.v_slots = v_grid; a.slots = 1; a.out_count = 1;
+    a.tv_out = tv_out; a.loss = loss_out;
+    bilagrid_tv_kernel<<<1, TV_THREADS, 0, s>>>(a);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_bilagrid_update_views(cudaStream_t s, float *grids, float *m, float *v, int32_t *steps, uint32_t num_views,
+                                         float lr, float tv_weight, float *v_slots, uint32_t slot_stride, const uint32_t *slot_view,
+                                         uint32_t view_stride, uint32_t slots, uint32_t out_begin, uint32_t out_count,
+                                         float *tv_out, float *loss_terms) {
+    if (slots == 0) return cudaSuccess;
+    TvArgs a;
+    a.grids = grids; a.m = m; a.v = v; a.steps = steps; a.num_views = num_views; a.lr = lr; a.tv_weight = tv_weight;
+    a.v_slots = v_slots; a.slot_view = slot_view; a.slot_stride = slot_stride; a.view_stride = view_stride; a.slots = slots;
+    a.out_begin = out_begin; a.out_count = out_count; a.tv_out = tv_out; a.loss = loss_terms;
+    bilagrid_tv_kernel<<<slots, TV_THREADS, 0, s>>>(a);
     return cudaGetLastError();
 }
 

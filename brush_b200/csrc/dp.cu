@@ -186,10 +186,22 @@ int dp_exchange_header(DpComm *cm, uint32_t local, const float *hdr, float *hdr_
     return a.AllGather(hdr, hdr_all, (size_t)local * 4, NCCL_FLOAT32, cm->comm, cm->stream);
 }
 
+int dp_exchange_grids(DpComm *cm, size_t floats, const float *send, float *recv) {
+    NcclApi &a = nccl();
+    const int rc = a.AllGather(send, recv, floats, NCCL_FLOAT32, cm->comm, cm->stream);
+    if (rc != 0) return rc;
+    return cudaEventRecord(cm->ev_chunk[2], cm->stream) == cudaSuccess ? 0 : -1;
+}
+
 // ---- small device helpers of the multi-view step
 __global__ void write_header_kernel(float *hdr, DpHeader h, uint32_t local) {
     const uint32_t i = threadIdx.x;
     if (i < local * 4) hdr[i] = (i & 3u) < 3u ? h.pos[i >> 2][i & 3u] : 0.0f;
+}
+
+__global__ void write_grid_index_kernel(float *slots, uint32_t stride, DpGridIndex idx, uint32_t local) {
+    const uint32_t i = threadIdx.x;
+    if (i < local) slots[(size_t)i * stride] = __uint_as_float(idx.view[i]);
 }
 
 // Folds one local view's gradients into the exchange buffers: small row (+)= (v_transforms, v_raw_opac, visible), the stat
@@ -271,6 +283,10 @@ cudaError_t launch_pack_color(cudaStream_t s, uint32_t n, uint32_t local, uint32
 
 cudaError_t launch_write_header(cudaStream_t s, float *hdr, const DpHeader &h, uint32_t local) {
     write_header_kernel<<<1, 64, 0, s>>>(hdr, h, local);
+    return cudaGetLastError();
+}
+cudaError_t launch_write_grid_index(cudaStream_t s, float *slots, uint32_t stride, const DpGridIndex &idx, uint32_t local) {
+    write_grid_index_kernel<<<1, DP_MAX_VIEWS, 0, s>>>(slots, stride, idx, local);
     return cudaGetLastError();
 }
 cudaError_t launch_pack_view(cudaStream_t s, uint32_t n, uint32_t local, uint32_t li, bool first, const float *v_t, const float *v_o,

@@ -11,6 +11,7 @@
 //       fold_min_scale (brush-render/src/gaussian_splats.rs:86-111): the Mip-Splatting 3D filter floor.
 #include <algorithm>
 
+#include "bg_adam.cuh"
 #include "bg_common.cuh"
 #include "bg_fold.cuh"
 #include "bg_rng.cuh"
@@ -22,31 +23,14 @@ namespace bg {
 // depend on the grid size.
 constexpr uint64_t GRID_CAP = 132ull * 16;
 
-struct AdamConsts {
-    float lr, beta1, beta2, eps, f1, f2, bc1, bc2;
-    int first;
-};
-
-__device__ __forceinline__ float adam_update(float p, float g, float &m, float v, const AdamConsts &k, float step) {
-    float m_hat = m / k.bc1;
-    float v_hat = v / k.bc2;
-    float upd = m_hat / (sqrtf(v_hat) + k.eps);
-    return p - upd * step;
-}
-
 __global__ void __launch_bounds__(256)
 adam_kernel(float *__restrict__ p, const float *__restrict__ g, float *__restrict__ m, float *__restrict__ v,
             uint64_t total, uint32_t cols, const float *__restrict__ lr_scale, AdamConsts k) {
     const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
         float gg = __ldg(g + i);
-        float mm = k.first ? gg * k.f1 : m[i] * k.beta1 + gg * k.f1;
-        float gsq = gg * gg;
-        float vv = k.first ? gsq * k.f2 : v[i] * k.beta2 + gsq * k.f2;
-        m[i] = mm;
-        v[i] = vv;
         float step = lr_scale ? __ldg(lr_scale + (uint32_t)(i % cols)) * k.lr : k.lr;
-        p[i] = adam_update(p[i], gg, mm, vv, k, step);
+        adam_element(p[i], gg, m[i], v[i], k, step);
     }
 }
 

@@ -22,7 +22,8 @@ provides memory, streams and (for N>1) torch.distributed.
                          start of refine() and recomputed at its end while progress < 0.9 (train.rs:437, 641-647).
 
   bilateral_grids       <- per-view appearance compensation (DESIGN.md section 4.11): step() and step_fused() slice the
-                         render by the view's grid before the loss and update that grid after the splats (bilagrid.py)
+                         render by the view's grid before the loss and update that grid after the splats (bilagrid.py);
+                         step_views_bilagrid() does the same for several views per step, on one device or sharded
 
 Out of scope here: LPIPS.
 """
@@ -547,18 +548,46 @@ class SplatTrainer:
             return st
         return self._step_views(batches, splats, group, chunks, distributed, with_depth=True)
 
-    def _step_views(self, batches, splats, group, chunks, distributed, with_depth: bool) -> TrainStepStats:
+    def step_views_bilagrid(self, batches: Sequence[SceneBatch], splats: Splats, group=None, chunks: int = 0,
+                            distributed: Optional[bool] = None) -> TrainStepStats:
+        """step_views (or step_views_depth, when batches carry depth and depth_loss_weight > 0) with the views' bilateral
+        grids (DESIGN.md section 4.11) through ONE ABI call (bg_train_step_views_bilagrid).  Each batch's view_index
+        selects its grid: the loss is taken on the view's render sliced by its grid, the splat gradient is the mean over
+        the views as in step_views, and every view of the step (across ranks too) takes one grid update -- a view that
+        appears more than once gets one update from the sum of its gradients.  The grids' step counts advance on the
+        device.  loss is the mean over this rank's views of image + depth + TV loss; tv_loss holds each local view's TV
+        term [local] (depth_loss / view_depth_losses as in step_views_depth when the batches carry depth), all on the
+        device, views of buffers the next step overwrites."""
+        grids = self.bilateral_grids
+        if grids is None:
+            raise ValueError("step_views_bilagrid needs TrainConfig(bilateral_grid=True) and SplatTrainer(..., bilateral_grids=)")
+        if grids.grids.device != self.ctx.device:
+            raise ValueError(f"the bilateral grids are on device {grids.grids.device}, the trainer renders on {self.ctx.device}")
+        for b in batches:
+            if b.view_index < 0:
+                raise ValueError("step_views_bilagrid needs SceneBatch.view_index on every batch (it selects the view's grid)")
+            grids.check_view(b.view_index)
+        has_depth = any(b.depth is not None for b in batches)
+        with_depth = has_depth and self.config.depth_loss_weight > 0.0
+        st = self._step_views(batches, splats, group, chunks, distributed, with_depth=with_depth, bilagrid=True)
+        if has_depth and not with_depth:
+            zeros = torch.zeros(len(batches), dtype=torch.float32, device=self.ctx.device)
+            st.depth_loss, st.view_depth_losses = zeros.sum(), zeros
+        return st
+
+    def _step_views(self, batches, splats, group, chunks, distributed, with_depth: bool, bilagrid: bool = False) -> TrainStepStats:
         import torch.distributed as dist
         cfg = self.config
-        if self.bilateral_grids is not None:
-            raise ValueError("step_views and step_views_depth do not train bilateral grids: use step() or step_fused()")
+        if self.bilateral_grids is not None and not bilagrid:
+            raise ValueError("step_views and step_views_depth do not train bilateral grids: use step_views_bilagrid(), step() "
+                             "or step_fused()")
         self._ensure_state(splats)
         dev = self.ctx.device
         lib = _lib.load()
         multi = dist.is_initialized() and dist.get_world_size(group) > 1 if distributed is None else bool(distributed)
         world = dist.get_world_size(group) if multi else 1
         local = len(batches)
-        who = "step_views_depth" if with_depth else "step_views"
+        who = "step_views_bilagrid" if bilagrid else "step_views_depth" if with_depth else "step_views"
         if local == 0 or local * world > 16:
             raise ValueError(f"{who} needs 1..16 views per step in total")
         if not with_depth and cfg.depth_loss_weight > 0.0 and any(b.depth is not None for b in batches):
@@ -580,7 +609,8 @@ class SplatTrainer:
         for b in batches:
             if b.img_size() != (img_h, img_w) or (b.has_alpha, b.masked_alpha) != (b0.has_alpha, b0.masked_alpha):
                 raise ValueError("the views of one step must share the image size and the alpha mode")
-        ws_bytes = lib.bg_train_step_views_depth_workspace_bytes if with_depth else lib.bg_train_step_views_workspace_bytes
+        ws_bytes = (lib.bg_train_step_views_bilagrid_workspace_bytes if bilagrid else
+                    lib.bg_train_step_views_depth_workspace_bytes if with_depth else lib.bg_train_step_views_workspace_bytes)
         need = int(ws_bytes(n, k, img_w, img_h, local, world))
         if self._views_ws is None or self._views_ws.numel() < need:
             self._views_ws = torch.empty(need, dtype=torch.uint8, device=dev)
@@ -588,6 +618,8 @@ class SplatTrainer:
         a, lr_mean, keep = self._views_args(batches, splats, self._views_ws, need, chunks)
         a.loss_out = self._views_loss.data_ptr()
         comm = self._dp_comm.handle if multi else None
+        if bilagrid:
+            return self._step_views_bilagrid(batches, targets, a, lr_mean, keep, comm, with_depth)
         if not with_depth:
             _lib.check(lib.bg_train_step_views(self.ctx.handle, comm, _stream_ptr(dev), C.byref(a)), "bg_train_step_views")
             self._views_keepalive = keep
@@ -600,6 +632,26 @@ class SplatTrainer:
         per_view = self._views_depth_loss[:local]
         return TrainStepStats(num_visible_event=None, lr_mean=lr_mean, loss=self._views_loss[0], depth_loss=per_view.mean(),
                               view_depth_losses=per_view)
+
+    def _step_views_bilagrid(self, batches, targets, a, lr_mean: float, keep, comm, with_depth: bool) -> TrainStepStats:
+        cfg, dev, lib = self.config, self.ctx.device, _lib.load()
+        grids = self.bilateral_grids
+        local = len(batches)
+        ds = None
+        if with_depth:
+            if self._views_depth_loss is None:
+                self._views_depth_loss = torch.zeros(16, dtype=torch.float32, device=dev)
+            ds = self._views_depth_args(batches, targets, self._views_depth_loss)
+        gv, idx = grids.views_args([b.view_index for b in batches], self._bilagrid_lr(), cfg.bilateral_grid_tv_weight,
+                                   grids.views_tv_loss)
+        _lib.check(lib.bg_train_step_views_bilagrid(self.ctx.handle, comm, _stream_ptr(dev), C.byref(a), ds, C.byref(gv)),
+                   "bg_train_step_views_bilagrid")
+        self._views_keepalive = (keep, targets, ds, idx)
+        st = TrainStepStats(num_visible_event=None, lr_mean=lr_mean, loss=self._views_loss[0], tv_loss=grids.views_tv_loss[:local])
+        if with_depth:
+            per_view = self._views_depth_loss[:local]
+            st.depth_loss, st.view_depth_losses = per_view.mean(), per_view
+        return st
 
     def _views_depth_args(self, batches, targets, losses: torch.Tensor):
         """The host array of BgDepthSupervision of step_views_depth: one per view, view i's depth loss into losses[i]."""

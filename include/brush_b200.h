@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define BG_ABI_VERSION 12u
+#define BG_ABI_VERSION 13u
 
 /* f32 lanes per projected splat: a 64-byte row, four aligned 128-bit loads.  Lanes 0..8 are the reference
  * layout (kernels/helpers.rs:49-53: xy_x, xy_y, conic_x, conic_y, conic_z, color_a, color_r, color_g, color_b).
@@ -613,6 +613,43 @@ uint64_t bg_train_step_views_depth_workspace_bytes(uint32_t n, uint32_t k, uint3
                                                    uint32_t world);
 int32_t bg_train_step_views_depth(BgContext *ctx, BgDpComm *comm, void *stream, BgTrainViewsArgs *args,
                                   const BgDepthSupervision *depth /* host [local_views] */);
+
+/* bg_train_step_views (or bg_train_step_views_depth when depth is non-null) with the views' bilateral grids (DESIGN.md
+ * section 4.11).  Local view i trains the grid of global training view view_index[i]: render -> bg_bilagrid_slice of the raw
+ * render -> image loss on the sliced image (the depth term, if any, on the raw alpha and depth) -> bg_bilagrid_slice_backward
+ * in place, the view's grid gradient into a slot of its own -> the blend backward replays the raw render -> the rest of the
+ * views step.  The splat gradient is the mean over the views and the splat exchange is unchanged; a grid gradient is the
+ * unscaled gradient of its view's loss (what bg_train_step_bilagrid computes for the same render).  With a communicator the
+ * slots and their view indices are all-gathered (behind the last local view's slice backward, under its blend and
+ * projection backward), and every rank runs the same grid update over all world * local_views slots in global order
+ * rank * local_views + i: each view of the step takes ONE update -- its slots' gradients summed in slot order, TV, then
+ * Adam (bit-identical to bg_bilagrid_update given that gradient, lr, tv_weight and step = steps[view] + 1) -- and
+ * steps[view] advances by 1 on the device.  The grids of views not in the step are untouched.  tv_loss_out[i] = tv_weight
+ * * TV of view_index[i]'s grid before the update (the same for every occurrence of a view).  *loss_out = mean over this
+ * rank's views of (image loss + L_d,i + tv_loss_out[i]).  Nothing is read back (capturable in a CUDA graph).
+ * workspace: bg_train_step_views_bilagrid_workspace_bytes (else BG_ERR_CAPACITY).  Checked before the first launch: null
+ * pointers are BG_ERR_NULL; grids, m, v not 16-byte aligned, steps not 4-byte aligned, num_views == 0, a negative or
+ * non-finite lr or tv_weight, or a view_index[i] >= num_views is BG_ERR_INVALID; every check of bg_train_step_views and
+ * bg_train_step_views_depth applies.
+ * bg_bilagrid_update_views: the grid update above on its own, for hosts that drive the operators: `slots` (1..16) gradient
+ * slots v_grids [slots][L,H,W,12] (16-byte aligned) of views slot_view [slots] (device; a view >= num_views is skipped),
+ * tv_loss_out [slots].  The first slot of each view receives the summed gradient + the TV gradient; view_index is not
+ * read. */
+typedef struct {
+    float *grids, *m, *v;          /* device [num_views][L,H,W,12] each, 16-byte aligned */
+    int32_t *steps;                /* device [num_views]: each view's grid step count, advanced on the device */
+    uint32_t num_views;
+    const uint32_t *view_index;    /* host [local_views]: global training-view index of each local view */
+    float lr, tv_weight;           /* the step's learning rate (the caller evaluates the schedule), the TV weight */
+    float *tv_loss_out;            /* device [local_views] (bg_bilagrid_update_views: [slots]) */
+} BgBilagridViews;
+uint64_t bg_train_step_views_bilagrid_workspace_bytes(uint32_t n, uint32_t k, uint32_t w, uint32_t h, uint32_t local_views,
+                                                      uint32_t world);
+int32_t bg_train_step_views_bilagrid(BgContext *ctx, BgDpComm *comm, void *stream, BgTrainViewsArgs *args,
+                                     const BgDepthSupervision *depth /* nullable, host [local_views] */,
+                                     const BgBilagridViews *grids);
+int32_t bg_bilagrid_update_views(BgContext *ctx, void *stream, const BgBilagridViews *grids, uint32_t slots,
+                                 const uint32_t *slot_view /* device [slots] */, float *v_grids /* [slots][L,H,W,12], += TV */);
 
 /* Building blocks of the exchange for hosts that drive the operators themselves.  The SH part of the
  * gradient of ONE view is rank one per Gaussian: v_sh[g,k,:] = Y_k(dir(mean_g, camera)) * v_color[g,:]

@@ -13,7 +13,8 @@
 //   image_loss_forward/backward <- LossOps                     brush-loss/src/lib.rs:718-733
 //   AdamScaled                  <- brush-train/src/adam_scaled.rs:64-165
 //   TrainConfig, SplatTrainer   <- brush-train/src/config.rs, train.rs:138-893: step (bg_train_step), step_views
-//                                  (bg_train_step_views: several views per step, one or several devices), refine (bg_refine)
+//                                  (bg_train_step_views: several views per step, one or several devices),
+//                                  step_views_bilagrid (the same with the views' bilateral grids), refine (bg_refine)
 //   BoundingBox, bounds_from_pos <- brush-render/src/bounding_box.rs, brush-train/src/splat_init.rs:130-160
 //   Splats                      <- brush-render/src/gaussian_splats.rs:57-74 (owns the three parameter tensors)
 //   DpComm                      <- no reference counterpart (SURVEY.md 8e): one NCCL rank per context, behind the ABI
@@ -459,13 +460,16 @@ inline double bilagrid_lr(double lr0, int n, uint32_t total_train_iters) {
 }
 
 // The bilateral grids of all training views (DESIGN.md section 4.11): grids [views, L, H, W, 12] uploaded at identity,
-// their Adam moments (zero) and the host-side per-view step counts.  A view's grid changes only in the steps that
-// render it.
+// their Adam moments (zero) and the per-view step counts.  A view's grid changes only in the steps that render it, and its
+// count is the number of those steps.  The counts are kept on the host (the single-view step advances them) and on the
+// device (the multi-view step advances them there); each copy is brought up to date from the other only after a step of
+// the other kind.
 class BilateralGrids {
    public:
     explicit BilateralGrids(uint32_t num_views, cudaStream_t s = nullptr)
         : views_(num_views), grids_((size_t)num_views * BG_BILAGRID_FLOATS), m_((size_t)num_views * BG_BILAGRID_FLOATS, true),
-          v_((size_t)num_views * BG_BILAGRID_FLOATS, true), tv_loss_(1, true), steps_(num_views, 0) {
+          v_((size_t)num_views * BG_BILAGRID_FLOATS, true), tv_loss_(1, true), views_tv_loss_(16, true), dsteps_(num_views, true),
+          steps_(num_views, 0) {
         if (num_views == 0) throw Error(BG_ERR_INVALID, "BilateralGrids: at least one view");
         std::vector<float> host((size_t)num_views * BG_BILAGRID_FLOATS, 0.0f);
         for (size_t c = 0; c < host.size(); c += 12) host[c] = host[c + 5] = host[c + 10] = 1.0f;   // M = I, b = 0
@@ -476,26 +480,54 @@ class BilateralGrids {
     float *grid(uint32_t view) { return grids_.data() + (size_t)check_view(view) * BG_BILAGRID_FLOATS; }
     float *m(uint32_t view) { return m_.data() + (size_t)check_view(view) * BG_BILAGRID_FLOATS; }
     float *v(uint32_t view) { return v_.data() + (size_t)check_view(view) * BG_BILAGRID_FLOATS; }
-    int steps(uint32_t view) const { return steps_[check_view(view)]; }
+    // the view's step count (reads the device counts back, synchronously, after multi-view steps)
+    int steps(uint32_t view) { return host_steps()[check_view(view)]; }
+    const int32_t *device_steps() const { return dsteps_.data(); }
     const float *tv_loss() const { return tv_loss_.data(); }   // device scalar of the last update
+    const float *views_tv_loss() const { return views_tv_loss_.data(); }   // device [local views] of the last multi-view step
     // Counts one more step of `view` and returns its BgBilagridStep
     BgBilagridStep step_args(uint32_t view, float lr, float tv_weight) {
+        check_view(view);
         BgBilagridStep b;
         b.grid = grid(view); b.m = m(view); b.v = v(view);
-        b.step = ++steps_[view];
+        b.step = ++host_steps()[view];
+        current_ = HOST;
         b.lr = lr; b.tv_weight = tv_weight;
         b.tv_loss_out = tv_loss_.data();
         return b;
     }
+    // The BgBilagridViews of a multi-view step whose counts advance on the device (uploads them once after single-view
+    // steps); view_index must outlive the call.
+    BgBilagridViews views_args(const std::vector<uint32_t> &view_index, float lr, float tv_weight, cudaStream_t s) {
+        for (uint32_t v : view_index) check_view(v);
+        if (current_ == HOST) dsteps_.upload(steps_.data(), steps_.size(), s);
+        current_ = DEVICE;
+        BgBilagridViews g;
+        g.grids = grids_.data(); g.m = m_.data(); g.v = v_.data(); g.steps = dsteps_.data();
+        g.num_views = views_; g.view_index = view_index.data();
+        g.lr = lr; g.tv_weight = tv_weight;
+        g.tv_loss_out = views_tv_loss_.data();
+        return g;
+    }
 
    private:
+    std::vector<int32_t> &host_steps() {
+        if (current_ == DEVICE) {
+            dsteps_.download(steps_.data(), steps_.size());
+            check_cuda(cudaStreamSynchronize(nullptr), "BilateralGrids step counts");
+            current_ = BOTH;
+        }
+        return steps_;
+    }
     uint32_t check_view(uint32_t view) const {
         if (view >= views_) throw Error(BG_ERR_INVALID, "BilateralGrids: view index out of range");
         return view;
     }
     uint32_t views_;
-    DeviceBuffer<float> grids_, m_, v_, tv_loss_;
-    std::vector<int> steps_;
+    DeviceBuffer<float> grids_, m_, v_, tv_loss_, views_tv_loss_;
+    DeviceBuffer<int32_t> dsteps_;
+    std::vector<int32_t> steps_;
+    enum { BOTH, HOST, DEVICE } current_ = BOTH;   // which copy of the counts is up to date
 };
 
 // brush-render/src/bounding_box.rs:5-31
@@ -757,20 +789,60 @@ class SplatTrainer {
         return {loss_.data(), views_depth_loss_.data()};
     }
 
+    // step_views with the views' bilateral grids (bg_train_step_views_bilagrid, DESIGN.md section 4.11): view_index[i] is
+    // camera i's training-view index (its grid); depth_targets / depth_valid_counts as in the depth overload, or both
+    // empty for no depth term.  Returns the device scalar of the loss (mean over this rank's views of image + depth + TV
+    // loss), the device float[local] of the views' depth losses (0 without a term) and of their TV terms.  Requires
+    // cfg.bilateral_grid.
+    struct GridViewsLosses {
+        const float *loss;
+        const float *depth_losses;
+        const float *tv_losses;
+    };
+    GridViewsLosses step_views_bilagrid(Context &ctx, DpComm *comm, cudaStream_t stream, const std::vector<Camera> &cameras,
+                                        const std::vector<const uint32_t *> &gt_packed, const std::vector<uint32_t> &view_index,
+                                        const std::vector<const float *> &depth_targets,
+                                        const std::vector<uint32_t> &depth_valid_counts, uint32_t w, uint32_t h, Splats &splats,
+                                        BilateralGrids &grids, const float *min_scale = nullptr, bool has_alpha = false,
+                                        bool masked_alpha = false) {
+        if (!cfg_.bilateral_grid) throw Error(BG_ERR_INVALID, "SplatTrainer::step_views_bilagrid: cfg.bilateral_grid is off");
+        const bool depth = !depth_targets.empty();
+        if (view_index.size() != cameras.size() ||
+            (depth && (depth_targets.size() != cameras.size() || depth_valid_counts.size() != cameras.size())))
+            throw Error(BG_ERR_INVALID, "SplatTrainer::step_views_bilagrid: one view index (and depth target and valid count) per camera");
+        std::vector<BgCamera> cams;
+        BgTrainViewsArgs a = views_args(comm, cameras, gt_packed, w, h, splats, min_scale, has_alpha, masked_alpha, cams, depth, nullptr, true);
+        const BgBilagridViews g = grids.views_args(view_index, (float)bilagrid_lr(cfg_.bilateral_grid_lr, step_, cfg_.total_train_iters),
+                                                   cfg_.bilateral_grid_tv_weight, stream);
+        std::vector<BgDepthSupervision> d(cameras.size());
+        for (size_t i = 0; depth && i < d.size(); i++) {
+            d[i].target = depth_targets[i];
+            d[i].weight = cfg_.depth_loss_weight;
+            d[i].valid_count = depth_targets[i] ? depth_valid_counts[i] : 0u;
+            d[i].depth_loss_out = views_depth_loss_.data() + i;
+        }
+        check(bg_train_step_views_bilagrid(ctx.handle(), comm ? comm->handle() : nullptr, stream, &a, depth ? d.data() : nullptr, &g),
+              "SplatTrainer::step_views_bilagrid");
+        if (!depth) check_cuda(cudaMemsetAsync(views_depth_loss_.data(), 0, cameras.size() * sizeof(float), stream), "SplatTrainer::step_views_bilagrid");
+        last_state_ = a.state_out;
+        return {loss_.data(), views_depth_loss_.data(), grids.views_tv_loss()};
+    }
+
    private:
     BgTrainViewsArgs views_args(DpComm *comm, const std::vector<Camera> &cameras, const std::vector<const uint32_t *> &gt_packed,
                                 uint32_t w, uint32_t h, Splats &splats, const float *min_scale, bool has_alpha, bool masked_alpha,
-                                std::vector<BgCamera> &cams, bool depth, const BilateralGrids *grids) {
-        // the multi-view steps have no grid term (DESIGN.md section 7)
-        if (grids) throw Error(BG_ERR_INVALID, "SplatTrainer::step_views: the multi-view step does not train bilateral grids");
-        refuse_grids("SplatTrainer::step_views");
+                                std::vector<BgCamera> &cams, bool depth, const BilateralGrids *grids, bool grid_step = false) {
+        // only step_views_bilagrid trains the grids
+        if (grids) throw Error(BG_ERR_INVALID, "SplatTrainer::step_views: the multi-view step does not train bilateral grids (step_views_bilagrid does)");
+        if (!grid_step) refuse_grids("SplatTrainer::step_views");
         const uint32_t local = (uint32_t)cameras.size(), world = comm ? (uint32_t)comm->world() : 1u;
         if (local == 0 || gt_packed.size() != cameras.size() || local * world > 16)
             throw Error(BG_ERR_INVALID, "SplatTrainer::step_views: 1..16 views per step in total, one image per camera");
         if (splats.n != n_ || splats.k != k_) throw Error(BG_ERR_INVALID, "SplatTrainer::step_views: splat count differs from the optimizer state");
         step_ += 1;
-        const uint64_t need = depth ? bg_train_step_views_depth_workspace_bytes(n_, k_, w, h, local, world)
-                                    : bg_train_step_views_workspace_bytes(n_, k_, w, h, local, world);
+        const uint64_t need = grid_step ? bg_train_step_views_bilagrid_workspace_bytes(n_, k_, w, h, local, world)
+                              : depth   ? bg_train_step_views_depth_workspace_bytes(n_, k_, w, h, local, world)
+                                        : bg_train_step_views_workspace_bytes(n_, k_, w, h, local, world);
         if (views_ws_.size() < need) views_ws_ = DeviceBuffer<unsigned char>(need);
         cams.resize(local);
         for (uint32_t i = 0; i < local; i++) cams[i] = make_uniforms(cameras[i], w, h);
