@@ -52,8 +52,10 @@ blend_bwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
     __shared__ __align__(16) float s_fact[RASTER_WARPS][2][WB * BFACT];  // post-reduction factors of the staged rows
 
     const uint32_t tile = blockIdx.x;
-    const uint32_t tid = threadIdx.x, lane = tid & 31u, wid = tid >> 5;
-    const uint32_t num_batches = __ldg(warp_batches + tile * RASTER_WARPS + wid);
+    // (warp index and batch count broadcast from lane 0: ptxas then knows the staging runs warp-converged, so the copy
+    // operands stay in uniform registers)
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, wid = __shfl_sync(0xffffffffu, tid >> 5, 0);
+    const uint32_t num_batches = __shfl_sync(0xffffffffu, __ldg(warp_batches + tile * RASTER_WARPS + wid), 0);
     BlendStage &st = s_stage[wid];
     if (lane == 0) { mbar_init(&st.bar[0], 1); mbar_init(&st.bar[1], 1); }
     __syncthreads();   // barriers initialised before any copy is issued
@@ -108,10 +110,11 @@ blend_bwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
 
     const size_t mbase = blend_mask_base(range_lo, tile) + wid;
     auto load_mask = [&](uint32_t b) -> uint32_t {
-        return b < num_batches ? __ldg(live_masks + mbase + (size_t)b * RASTER_WARPS) : 0u;
+        // (broadcast from lane 0: a mask ptxas knows is warp-uniform keeps the copy issue in uniform registers)
+        return __shfl_sync(0xffffffffu, b < num_batches ? __ldg(live_masks + mbase + (size_t)b * RASTER_WARPS) : 0u, 0);
     };
     // stage the rows of batch b selected by mask m, compacted in list order, into buffer b&1: the lanes park the row
-    // ids, one elected lane issues the TMA copies
+    // ids, the warp issues the TMA copies
     // (DEPTH: the same lane also starts the load of the row's z, which lands during the TMA wait)
     float z_next = 0.0f;
     auto stage = [&](uint32_t b, uint32_t m) -> uint32_t {

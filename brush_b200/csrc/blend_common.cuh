@@ -1,9 +1,10 @@
 // blend_common.cuh -- the blend kernels (blend_fwd.cu, blend_bwd.cu): shared layout, staging and the pair tests.
 //
-// Tile = 16x16 pixels = one CTA of 4 warps.  Warp k owns the 8x8 pixel block with origin (8*(k&1), 8*(k>>1)); lane l
-// owns the two pixels (l&7, l>>3) and (l&7, (l>>3)+4) of the block.  Every warp walks the tile's depth-ordered splat
-// list on its own, in batches of 32 splats, with no block-wide barrier inside the loop: a warp whose 64 pixels are
-// saturated retires at once, and the next batch's rows are staged while the current batch is blended.
+// Tile = 16x16 pixels = one CTA of 4 pixel warps (the forward adds a producer warp, blend_fwd.cu).  Warp k owns the 8x8
+// pixel block with origin (8*(k&1), 8*(k>>1)); lane l owns the two pixels (l&7, l>>3) and (l&7, (l>>3)+4) of the
+// block.  Every pixel warp walks the tile's depth-ordered splat list on its own, in batches of 32 splats, with no
+// block-wide barrier inside the loop: a warp whose 64 pixels are saturated stops blending at once, and later batches'
+// rows are staged while the current batch is blended.
 //
 //  * paired FP32.  The two pixels of a lane run ONE instruction stream, so all per-pixel arithmetic is
 //    written on float2 (fadd2_rn / fmul2_rn / ffma2_rn of bg_common.cuh; per-splat scalars are broadcast), and
@@ -35,7 +36,7 @@ constexpr int RASTER_THREADS = RASTER_WARPS * 32;
 constexpr int WB = 32;                    // splats per warp batch
 constexpr int ROW = BG_PROJECTED_STRIDE;  // 16 floats
 constexpr int ROW_PT = 12;                // lane of ln(255 opacity), the block-cull threshold
-constexpr int ROW_Z = 13;                 // pad lane that the DEPTH variants fill with the splat's camera-space z
+constexpr int ROW_Z = 13;                 // pad lane that the DEPTH backward fills with the splat's camera-space z
 
 struct BlendUniforms {
     uint32_t tiles_x, img_w, img_h;
@@ -53,11 +54,32 @@ __device__ __forceinline__ size_t blend_mask_base(uint32_t range_lo, uint32_t ti
 // ---- TMA staging of a batch of projected rows (north_star: "TMA staging of each tile's sorted Gaussian slice").
 // A tile's slice is an index list, not a contiguous range, and sm_90 has no gather form of the tensor copy, so every
 // 64-byte row is its own 1-D bulk copy (cp.async.bulk, SASS UBLKCP; 16-byte alignment on both sides, which the
-// 64-byte rows meet -- a 2-D tensor copy would need 128-byte aligned shared destinations).  One elected lane issues
-// the batch's copies against one mbarrier (complete_tx), the other lanes only park the row ids in shared memory
-// first; nothing occupies the LSU pipe or the register file for the copy.
+// 64-byte rows meet -- a 2-D tensor copy would need 128-byte aligned shared destinations).  The warp issues a batch's
+// copies against one mbarrier (complete_tx); nothing occupies the LSU pipe or the register file for the copy.
 //
-// Per-warp staging state: two buffers of 32 dense 64-byte rows, the ids of the rows in flight, one mbarrier each.
+// Issues the copies of rows 0..count) into the dense rows at `dst`, completing on `bar`: lane r holds the id of row r.
+// Call with the whole warp converged and `count` warp-uniform; the caller has armed `bar` with the bytes.  The id is
+// broadcast with a shuffle from a constant lane (the loop is unrolled), so ptxas knows every copy operand is
+// warp-uniform: the address is formed in uniform registers and the copy issues once per warp (elect.sync), with no
+// per-row ELECT waterfall -- 9 instructions per row, against 14 for one lane walking ids parked in shared memory.
+__device__ __forceinline__ void issue_rows_tma(float *dst, uint32_t id, uint32_t count, const float *projected,
+                                               unsigned long long *bar) {
+    const uint32_t d0 = smem_u32(dst), b = smem_u32(bar);
+#pragma unroll
+    for (uint32_t r = 0; r < WB; r++) {
+        if (r >= count) break;
+        const float *src = projected + (size_t)__shfl_sync(0xffffffffu, id, r) * ROW;
+        asm volatile(
+            "{\n.reg .pred p;\nelect.sync _|p, 0xffffffff;\n"
+            "@p cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n}" ::"r"(
+                d0 + r * (ROW * 4u)),
+            "l"(src), "n"(ROW * 4), "r"(b)
+            : "memory");
+    }
+}
+
+// Per-warp staging state of the backward: two buffers of 32 dense 64-byte rows, the compacted ids of the rows in
+// flight, one mbarrier each.
 struct __align__(128) BlendStage {
     float rows[2][WB * ROW];
     uint32_t ids[2][WB];
@@ -65,17 +87,16 @@ struct __align__(128) BlendStage {
 };
 
 // Issues the copy of `count` rows (ids already compacted in st.ids[buf][0..count)) into st.rows[buf].  Call with the
-// whole warp converged; returns after the elected lane has issued.  The lanes wrote per-splat constants into the rows
-// of this buffer with generic stores when it was last consumed; the async-proxy copies overwrite them, so every lane
-// fences its generic writes against the async proxy before the warp hands the buffer to the elected lane.
+// whole warp converged and `count` warp-uniform.  The lanes wrote per-splat constants into the rows of this buffer
+// with generic stores when it was last consumed; the async-proxy copies overwrite them, so every lane fences its
+// generic writes against the async proxy before the warp issues.
 __device__ __forceinline__ void stage_rows_tma(BlendStage &st, uint32_t buf, uint32_t count, const float *projected, uint32_t lane) {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    __syncwarp();   // ids and the fenced writes visible to the elected lane
-    if (lane == 0 && count > 0) {
-        mbar_expect_tx(&st.bar[buf], count * (ROW * 4u));
-        for (uint32_t r = 0; r < count; r++)
-            tma_bulk_g2s(&st.rows[buf][r * ROW], projected + (size_t)st.ids[buf][r] * ROW, ROW * 4u, &st.bar[buf]);
-    }
+    __syncwarp();   // ids and the fenced writes visible to every lane
+    if (count == 0) return;
+    const uint32_t id = st.ids[buf][lane];   // (stale past count: never read)
+    if (lane == 0) mbar_expect_tx(&st.bar[buf], count * (ROW * 4u));
+    issue_rows_tma(st.rows[buf], id, count, projected, &st.bar[buf]);
 }
 
 // True when the splat may contribute to some pixel centre of the rectangle [x0,x1] x [y0,y1].

@@ -7,30 +7,98 @@
 // past the last blended splat (rasterize.rs:183-189), and the hand-off words of blend_common.cuh.
 // SMOOTH (test-only, BWD_INFO only): the smooth alpha cutoff of blend_common.cuh, and its wider block-cull margin.
 // DEPTH (BWD_INFO only): also the accumulated depth D = sum vis_i z_i ([h,w] f32, no background term; DESIGN §4.6),
-// z_i = depths[compact id], the depth-sort key.  The staging lane parks z_i in pad lane 13 of the row; every other
+// z_i = depths[compact id], the depth-sort key.  The producer lanes store z_i in the ring slot's z table; every other
 // output (image, visible, trimmed ends, hand-off words) is the same as without DEPTH.
 //
 // Bound: instruction issue (FP32 + MUFU), not HBM.  Per warp-splat iteration (64 pixel-splat pairs) the loop is
-// 3 broadcast LDS.128, 4 scalar + 9 paired (18 scalar) FMA-pipe operations, 2 MUFU.EX2 and the pair tests.  The rows of a
-// batch are staged by TMA (per-row bulk copies, blend_common.cuh) into the warp's double buffer.
+// 3 broadcast LDS.128, 4 scalar + 9 paired (18 scalar) FMA-pipe operations, 3 colour clamps, 2 MUFU.EX2 and the pair
+// tests.  The rows of a batch are staged once per tile by TMA (per-row bulk copies, blend_common.cuh) into a ring the
+// four pixel warps share (below).
 #include "blend_common.cuh"
 #include "bg_launch.cuh"
 
 namespace bg {
 
+// ---- the tile's ring of staged batches.  Batch b of the tile's list lives in slot b % FWD_RING.  full[k]: the
+// producer's arrive + the transaction bytes of the slot's copies; empty[k]: one arrival per pixel warp that is done
+// reading the slot.  The pixel warps only read the ring (the colour clamp is applied where the colour is used), so
+// every row is staged once per tile instead of once per warp.
+constexpr int FWD_RING = 4;
+constexpr int FWD_THREADS = RASTER_THREADS + 32;   // four pixel warps + the producer warp
+struct __align__(128) BlendRing {
+    float rows[FWD_RING][WB * ROW];
+    float z[FWD_RING][WB];   // DEPTH: the rows' camera-space z, stored by the producer lanes
+    unsigned long long full[FWD_RING], empty[FWD_RING];
+};
+
+__device__ __forceinline__ void mbar_arrive(unsigned long long *bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+__device__ __forceinline__ bool mbar_try_wait(unsigned long long *bar, uint32_t parity) {
+    uint32_t ok;
+    asm volatile(
+        "{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}"
+        : "=r"(ok)
+        : "r"(smem_u32(bar)), "r"(parity)
+        : "memory");
+    return ok != 0u;
+}
+
 template <bool BWD_INFO, bool SMOOTH, bool DEPTH>
-__global__ void __launch_bounds__(RASTER_THREADS)
+__global__ void __launch_bounds__(FWD_THREADS)
 blend_fwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict__ cgid_from_isect,
                  uint32_t *__restrict__ tile_offsets, const uint32_t *__restrict__ gid_from_cgid,
                  float4 *__restrict__ out_f32, uint32_t *__restrict__ out_packed, float *__restrict__ visible,
                  uint32_t *__restrict__ live_masks, uint32_t *__restrict__ warp_batches, BlendUniforms u,
                  const float *__restrict__ depths, float *__restrict__ out_depth) {
-    __shared__ BlendStage s_stage[RASTER_WARPS];   // per warp, double buffered
+    __shared__ BlendRing s_ring;
     __shared__ uint32_t s_max_useful;
+    __shared__ uint32_t s_live;   // bit k: pixel warp k still blends (clears when all its pixels are saturated)
+    __shared__ uint32_t s_end;    // batches the producer issued; lowered from num_batches when it stops early
 
     const uint32_t tile = blockIdx.x;
-    const uint32_t tid = threadIdx.x, lane = tid & 31u, wid = tid >> 5;
+    // (the warp index broadcast from lane 0: ptxas then knows the producer's branch is warp-uniform, so its copy
+    // operands stay in uniform registers)
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, wid = __shfl_sync(0xffffffffu, tid >> 5, 0);
     const uint32_t tile_x0 = (tile % u.tiles_x) * TILE_W, tile_y0 = (tile / u.tiles_x) * TILE_W;
+    const uint32_t range_lo = tile_offsets[tile * 2], range_hi = tile_offsets[tile * 2 + 1];
+    const uint32_t num_batches = (range_hi - range_lo + WB - 1) / WB;
+    if (tid < FWD_RING) { mbar_init(&s_ring.full[tid], 1); mbar_init(&s_ring.empty[tid], RASTER_WARPS); }
+    if (tid == 0) {
+        s_max_useful = range_lo;
+        s_end = num_batches;
+        // a warp whose pixels are all outside the image has nothing to blend: it counts as retired from the start
+        uint32_t live = 0;
+        for (uint32_t k = 0; k < RASTER_WARPS; k++)
+            if (tile_x0 + 8u * (k & 1u) < u.img_w && tile_y0 + 8u * (k >> 1) < u.img_h) live |= 1u << k;
+        s_live = live;
+    }
+    __syncthreads();   // barriers initialised before any copy is issued
+
+    if (wid == RASTER_WARPS) {
+        // ---- producer: the lanes load a batch's ids coalesced, the warp issues its copies once for all four warps
+        uint32_t b = 0;
+        for (; b < num_batches; b++) {
+            const uint32_t slot = b % FWD_RING;
+            if (b >= FWD_RING) mbar_wait(&s_ring.empty[slot], (b / FWD_RING - 1u) & 1u);
+            if (__shfl_sync(0xffffffffu, *(volatile uint32_t *)&s_live, 0) == 0u) break;   // every pixel warp retired
+            const uint32_t start = range_lo + b * WB;
+            const uint32_t count = __shfl_sync(0xffffffffu, min((uint32_t)WB, range_hi - start), 0);
+            const uint32_t id = lane < count ? __ldg(cgid_from_isect + start + lane) : 0u;
+            if constexpr (DEPTH) {
+                s_ring.z[slot][lane] = lane < count ? __ldg(depths + id) : 0.0f;
+                __syncwarp();   // the z of the slot written before the arrive below releases it
+            }
+            if (lane == 0) mbar_expect_tx(&s_ring.full[slot], count * (ROW * 4u));
+            issue_rows_tma(s_ring.rows[slot], id, count, projected, &s_ring.full[slot]);
+        }
+        if (b < num_batches && lane == 0) *(volatile uint32_t *)&s_end = b;
+        // never leave a copy in flight: wait for the last batch issued into each slot
+        for (uint32_t k = b > (uint32_t)FWD_RING ? b - FWD_RING : 0u; k < b; k++)
+            mbar_wait(&s_ring.full[k % FWD_RING], (k / FWD_RING) & 1u);
+        return;
+    }
+
     const uint32_t blk_x0 = tile_x0 + 8u * (wid & 1u), blk_y0 = tile_y0 + 8u * (wid >> 1);
     const uint32_t pix_x = blk_x0 + (lane & 7u), pix_y0 = blk_y0 + (lane >> 3), pix_y1 = pix_y0 + 4u;
     const bool inside0 = pix_x < u.img_w && pix_y0 < u.img_h;
@@ -40,13 +108,6 @@ blend_fwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
     // rectangle of this warp's pixel centres
     const float rx0 = (float)blk_x0 + 0.5f, rx1 = rx0 + 7.0f, ry0 = (float)blk_y0 + 0.5f, ry1 = ry0 + 7.0f;
 
-    const uint32_t range_lo = tile_offsets[tile * 2], range_hi = tile_offsets[tile * 2 + 1];
-    if (BWD_INFO && tid == 0) s_max_useful = range_lo;
-    BlendStage &st = s_stage[wid];
-    if (lane == 0) { mbar_init(&st.bar[0], 1); mbar_init(&st.bar[1], 1); }
-    __syncthreads();   // barriers initialised before any copy is issued
-    uint32_t phase_bits = 0u;   // bit b: parity the next wait on buffer b expects
-
     // T2: transmittance of the blended prefix (what the output uses).  Tt2: the same value while the pixel is alive;
     // the stopping splat's T' (<= 1e-4) afterwards, so that "T' > 1e-4" alone rejects every later splat.
     float2 T2 = make_float2(1.0f, 1.0f);
@@ -54,48 +115,27 @@ blend_fwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
     float2 r2 = make_float2(0.0f, 0.0f), g2 = r2, b2 = r2, d2 = r2;
     uint32_t last_useful = range_lo;
 
-    const uint32_t num_batches = (range_hi - range_lo + WB - 1) / WB;
     const size_t mbase = blend_mask_base(range_lo, tile) + wid;
     uint32_t batches_walked = 0;
-    uint32_t next_id = 0;
-    float next_z = 0.0f;
-    // stage batch b: every lane parks the id of "its" list entry, one elected lane issues the TMA copies
-    auto prefetch = [&](uint32_t b) {
-        const uint32_t start = range_lo + b * WB;
-        const uint32_t count = min((uint32_t)WB, range_hi - start);
-        const uint32_t id = lane < count ? __ldg(cgid_from_isect + start + lane) : 0u;
-        next_id = id;
-        if constexpr (DEPTH) next_z = lane < count ? __ldg(depths + id) : 0.0f;   // in flight during the TMA wait
-        if (lane < count) st.ids[b & 1u][lane] = id;
-        stage_rows_tma(st, b & 1u, count, projected, lane);
-    };
-    // a warp whose pixels are all outside the image has nothing to blend
-    if (num_batches > 0 && __any_sync(0xffffffffu, inside0 || inside1)) {
-        prefetch(0);
-        for (uint32_t b = 0; b < num_batches; b++) {
+    uint32_t b = 0;
+    if ((s_live >> wid) & 1u) {
+        for (; b < num_batches; b++) {
+            const uint32_t slot = b % FWD_RING;
             const uint32_t batch_start = range_lo + b * WB;
             const uint32_t count = min((uint32_t)WB, range_hi - batch_start);
-            const uint32_t my_id = next_id;
-            const float my_z = next_z;
-            if (b + 1 < num_batches) prefetch(b + 1);
-            mbar_wait(&st.bar[b & 1u], (phase_bits >> (b & 1u)) & 1u);
-            phase_bits ^= 1u << (b & 1u);
-            float *rows = st.rows[b & 1u];
+            uint32_t my_id = 0;
+            if (BWD_INFO && lane < count) my_id = __ldg(cgid_from_isect + batch_start + lane);   // lands during the wait
+            mbar_wait(&s_ring.full[slot], (b / FWD_RING) & 1u);
+            const float *rows = s_ring.rows[slot];
             bool hit = false;
             if (lane < count) {
-                float *mine = rows + lane * ROW;
+                const float *mine = rows + lane * ROW;
                 const float4 A = *reinterpret_cast<const float4 *>(mine);
-                const float4 B = *reinterpret_cast<const float4 *>(mine + 4);
-                const float bcol = mine[8];
                 float pt = mine[ROW_PT];
                 if constexpr (SMOOTH) pt += SMOOTH_THR_EXTRA;
-                hit = block_may_hit(A.x, A.y, A.z, A.w, B.x, pt, rx0, rx1, ry0, ry1);
-                // per-splat constants are formed once here, by the lane that staged the row: colour -> max(colour, 0)
-                *reinterpret_cast<float2 *>(mine + 6) = make_float2(fmaxf(B.z, 0.0f), fmaxf(B.w, 0.0f));
-                mine[8] = fmaxf(bcol, 0.0f);
-                if constexpr (DEPTH) mine[ROW_Z] = my_z;
+                hit = block_may_hit(A.x, A.y, A.z, A.w, mine[4], pt, rx0, rx1, ry0, ry1);
             }
-            uint32_t bits = __ballot_sync(0xffffffffu, hit);   // (also orders the row fix-ups before the reads below)
+            uint32_t bits = __ballot_sync(0xffffffffu, hit);
             uint32_t used_m = 0, acted_m = 0;
             while (bits) {
                 const uint32_t s = (uint32_t)__ffs(bits) - 1u;
@@ -123,10 +163,10 @@ blend_fwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
                 // not apply), each lane remembers which splats touched its pixels, and "all pixels saturated" is
                 // checked once per batch (saturated pixels ignore the remaining splats of the batch).
                 const float2 vis = fmul2_rn(make_float2(c0 ? a0 : 0.0f, c1 ? a1 : 0.0f), T2);
-                r2 = ffma2_rn(bcast2(B.z), vis, r2);
-                g2 = ffma2_rn(bcast2(B.w), vis, g2);
-                b2 = ffma2_rn(bcast2(C.x), vis, b2);
-                if constexpr (DEPTH) d2 = ffma2_rn(bcast2(row[ROW_Z]), vis, d2);
+                r2 = ffma2_rn(bcast2(fmaxf(B.z, 0.0f)), vis, r2);
+                g2 = ffma2_rn(bcast2(fmaxf(B.w, 0.0f)), vis, g2);
+                b2 = ffma2_rn(bcast2(fmaxf(C.x, 0.0f)), vis, b2);
+                if constexpr (DEPTH) d2 = ffma2_rn(bcast2(s_ring.z[slot][s]), vis, d2);
                 const uint32_t bit = 1u << s;
                 // the hand-off needs the splats that changed a live pixel: blended it or stopped it
                 const bool acted = (Tt2.x > 1.0e-4f && act0) || (Tt2.y > 1.0e-4f && act1);
@@ -137,7 +177,8 @@ blend_fwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
                 Tt2.x = act0 ? nT.x : Tt2.x;
                 Tt2.y = act1 ? nT.y : Tt2.y;
             }
-            const uint32_t used = __reduce_or_sync(0xffffffffu, used_m);
+            const uint32_t used = __reduce_or_sync(0xffffffffu, used_m);   // (every lane is done reading the slot)
+            if (lane == 0) mbar_arrive(&s_ring.empty[slot]);
             if (BWD_INFO) {
                 const uint32_t acted = __reduce_or_sync(0xffffffffu, acted_m);
                 if (lane == 0) live_masks[mbase + (size_t)b * RASTER_WARPS] = acted;
@@ -148,11 +189,21 @@ blend_fwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
             }
             batches_walked = b + 1;
             if (__all_sync(0xffffffffu, !(Tt2.x > 1.0e-4f) && !(Tt2.y > 1.0e-4f))) {
-                if (b + 1 < num_batches) mbar_wait(&st.bar[(b + 1) & 1u], (phase_bits >> ((b + 1) & 1u)) & 1u);   // never leave a copy in flight
+                b++;
+                if (lane == 0) atomicAnd(&s_live, ~(1u << wid));
                 break;
             }
-            __syncwarp();  // all lanes are done with this buffer before the next prefetch overwrites its twin
         }
+    }
+    // retired: stop blending, but keep releasing the slots of the batches the producer still issues, until it has
+    // stopped (s_end) or the list ends
+    for (; b < num_batches; b++) {
+        const uint32_t slot = b % FWD_RING;
+        bool staged;
+        while (!(staged = mbar_try_wait(&s_ring.full[slot], (b / FWD_RING) & 1u)))
+            if (b >= *(volatile uint32_t *)&s_end) break;
+        if (__shfl_sync(0xffffffffu, (uint32_t)staged, 0) == 0u) break;
+        if (lane == 0) mbar_arrive(&s_ring.empty[slot]);
     }
 
     auto write_pixel = [&](float T, float r, float g, float bl, float d, uint32_t pix_y) {
@@ -173,12 +224,12 @@ blend_fwd_kernel(const float *__restrict__ projected, const uint32_t *__restrict
     if (inside1) write_pixel(T2.y, r2.y, g2.y, b2.y, d2.y, pix_y1);
     if (BWD_INFO) {
         if (lane == 0) warp_batches[tile * RASTER_WARPS + wid] = batches_walked;
-        // one block barrier, after all blending: publish the trimmed range end
+        // one barrier of the four pixel warps (named barrier 1; the producer has left), after all blending: publish
+        // the trimmed range end
         uint32_t m = last_useful;
         for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
-        __syncthreads();
         if (lane == 0 && m > range_lo) atomicMax(&s_max_useful, m);
-        __syncthreads();
+        asm volatile("bar.sync 1, %0;" ::"n"(RASTER_THREADS) : "memory");
         if (tid == 0) tile_offsets[tile * 2 + 1] = s_max_useful;
     }
 }
@@ -190,7 +241,7 @@ cudaError_t launch_blend_fwd(cudaStream_t s, bool bwd_info, bool smooth, uint32_
     BlendUniforms u;
     u.tiles_x = tiles_x; u.img_w = w; u.img_h = h; u.bg_r = bg[0]; u.bg_g = bg[1]; u.bg_b = bg[2];
 #define BG_LAUNCH_FWD(B, S, D, F32, PACKED, LM, WBAT)                                                                    \
-    blend_fwd_kernel<B, S, D><<<num_tiles, RASTER_THREADS, 0, s>>>(projected, cgid_from_isect, tile_offsets, gid_from_cgid, \
+    blend_fwd_kernel<B, S, D><<<num_tiles, FWD_THREADS, 0, s>>>(projected, cgid_from_isect, tile_offsets, gid_from_cgid, \
                                                                    F32, PACKED, visible, LM, WBAT, u, depths, out_depth)
     if (!bwd_info)
         BG_LAUNCH_FWD(false, false, false, nullptr, (uint32_t *)out_img, nullptr, nullptr);
