@@ -36,7 +36,6 @@ constexpr int RASTER_THREADS = RASTER_WARPS * 32;
 constexpr int WB = 32;                    // splats per warp batch
 constexpr int ROW = BG_PROJECTED_STRIDE;  // 16 floats
 constexpr int ROW_PT = 12;                // lane of ln(255 opacity), the block-cull threshold
-constexpr int ROW_Z = 13;                 // pad lane that the DEPTH backward fills with the splat's camera-space z
 
 struct BlendUniforms {
     uint32_t tiles_x, img_w, img_h;
@@ -79,10 +78,13 @@ __device__ __forceinline__ void issue_rows_tma(float *dst, uint32_t id, uint32_t
 }
 
 // Per-warp staging state of the backward: two buffers of 32 dense 64-byte rows, the compacted ids of the rows in
-// flight, one mbarrier each.
+// flight (read again by the gradient flush), the rows' camera-space z (DEPTH), each lane's constant flush factor, one
+// mbarrier each.
 struct __align__(128) BlendStage {
     float rows[2][WB * ROW];
     uint32_t ids[2][WB];
+    float z[2][WB];
+    float fconst[WB];
     unsigned long long bar[2];
 };
 
